@@ -402,10 +402,11 @@ __global__ void __launch_bounds__(32 * kStreamWarps) bloom_down2x_stream_kernel(
 
 // TM: -1 = no tone map, otherwise the tone-mapping operator (a compile-time parameter: one operator's code per instantiation, and its
 // per-frame constants - exposure scale, white-point normalisation - are hoisted out of the row loop by the compiler).
-// One warp's share: output columns [fx0, fx0 + 32) x rows [fyb, fye), fyb even; y1 = end of the caller's row range.
+// One warp's share: output columns [fx0, fx0 + 32) x rows [fyb, fye), fyb even; [ylo, y1) = the caller's row range (ylo may be odd: the
+// quad row it starts in is computed, its first row is not written).
 template <bool COMPOSITE, int TM, bool CG>
 __device__ __forceinline__ void up2x_stream_item(const dfx_bloom_attribs& A, const View<const float4>& fine, const View<const float4>& coarser, const View<float4>& out,
-                                                 int fx0, int fyb, int fye, int y1, int lane, const ToneMapIn& tm)
+                                                 int fx0, int fyb, int fye, int ylo, int y1, int lane, const ToneMapIn& tm)
 {
     const int   x = fx0 + lane;
     const bool  xin = x < out.w;
@@ -421,7 +422,7 @@ __device__ __forceinline__ void up2x_stream_item(const dfx_bloom_attribs& A, con
     auto hfilter = [&](float3 c) { return shfl3(c, s0) * w0 + shfl3(c, s0 + 1) * w1 + shfl3(c, s0 + 2) * w2 + shfl3(c, s0 + 3) * w3; }; // horizontal 4-tap
     auto load_fine = [&](int y) { return (xin && y < y1) ? ld(&fine.at(x, y)) : make_float4(0.f, 0.f, 0.f, 0.f); };
     auto emit = [&](int y, float3 s, float4 f) {
-        if (!xin || y >= y1) return;
+        if (!xin || y < ylo || y >= y1) return;
         const float3 c = xyz(f); // linear sampler at the texel centre == the texel
         if (COMPOSITE)
         {
@@ -461,9 +462,9 @@ __global__ void __launch_bounds__(32 * kStreamWarps) bloom_up2x_stream_kernel(df
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int fx0 = (blockIdx.x * kStreamWarps + warp) * 32;
-    const int fyb = y0 + blockIdx.y * (2 * coarse_rows_per_warp), fye = min(fyb + 2 * coarse_rows_per_warp, y1); // y0 is even (checked by the caller)
+    const int fyb = (y0 & ~1) + blockIdx.y * (2 * coarse_rows_per_warp), fye = min(fyb + 2 * coarse_rows_per_warp, y1); // whole quad rows
     if (fx0 >= out.w || fyb >= fye) return; // warp-uniform
-    up2x_stream_item<COMPOSITE, TM, false>(A, fine, coarser, out, fx0, fyb, fye, y1, lane, tm);
+    up2x_stream_item<COMPOSITE, TM, false>(A, fine, coarser, out, fx0, fyb, fye, y0, y1, lane, tm);
 }
 
 // =====================================================================================================================
@@ -641,7 +642,7 @@ __global__ void __launch_bounds__(kLevelsThreads, 3) bloom_levels_kernel(const _
             for (int item = gwarp; item < cols * chunks; item += nwarps)
             {
                 const int c = item % cols, r = item / cols;
-                up2x_stream_item<false, -1, true>(A, as_const(same), as_const(lo), out, c * 32, 2 * r * cpw, min(2 * (r + 1) * cpw, out.h), out.h, lane, tm);
+                up2x_stream_item<false, -1, true>(A, as_const(same), as_const(lo), out, c * 32, 2 * r * cpw, min(2 * (r + 1) * cpw, out.h), 0, out.h, lane, tm);
             }
         }
         else
@@ -750,12 +751,15 @@ static dfx_status launch_up(void* stream, int mode, const dfx_bloom_attribs& A, 
                             dfx_rows rows, const ToneMapIn& tm)
 {
     cudaStream_t s     = as_stream(stream);
-    const bool   exact = out.w == 2 * lo.w && out.h == 2 * lo.h && (rows.y0 & 1) == 0;
-    const int    impl  = bloom_impl();
-    if (mode == 2 && !exact) return set_error(DFX_ERR_UNSUPPORTED, "fused composite+tonemap needs an exact 2:1 level");
-    if (exact && impl == 1)
+    const bool   exact2 = out.w == 2 * lo.w && out.h == 2 * lo.h;
+    const bool   exact  = exact2 && (rows.y0 & 1) == 0;
+    const int    impl   = bloom_impl();
+    if (mode == 2 && !exact) return set_error(DFX_ERR_UNSUPPORTED, "fused composite+tonemap needs an exact 2:1 level and an even first row");
+    // The streaming kernel also takes a range that starts at an odd row (it computes that row's quad and skips the row above), so
+    // that the rows of a partial call are bit-identical to the same rows of a whole-level call. The tile kernels need an even y0.
+    if (exact2 && impl == 1)
     {
-        const int bx = div_up(out.w, 32 * kStreamWarps), n = div_up(rows.y1 - rows.y0, 2); // coarse rows
+        const int bx = div_up(out.w, 32 * kStreamWarps), n = div_up(rows.y1 - (rows.y0 & ~1), 2); // coarse rows
         // coarse rows per warp: dfx_tune("bloom_up_rows"), 0 = as few as fill one wave. Unlike the down-sampling, short warps win here.
         const int fixed_rows = dfx_tune_get("bloom_up_rows", 4);
 #define DFX_UP_LAUNCH(COMP, TMODE)                                                                                                                   \

@@ -539,7 +539,8 @@ DFX_API dfx_status dfx_pass_tonemap(void* stream, const dfx_tonemap_attribs* att
 /* Fused variants (an element-wise pass is evaluated inside the kernel that consumes / produces its plane, so the
  * intermediate frame never makes a round trip through HBM). Same arithmetic per pixel as the separate passes.
  *   compose + T1 : `color` is the un-composed scene colour; the composed colour is computed on the fly.
- *   B4 + M1/M2   : writes the tone-mapped LDR frame directly; only for exact 2:1 levels (DFX_ERR_UNSUPPORTED otherwise). */
+ *   B4 + M1/M2   : writes the tone-mapped LDR frame directly; only for exact 2:1 levels and an even rows.y0
+ *                  (DFX_ERR_UNSUPPORTED otherwise). */
 DFX_API dfx_status dfx_pass_compose_taa(void* stream, const dfx_camera_attribs* cameras_dev, const dfx_taa_attribs* attribs, uint32_t flags,
                                         const dfx_plane* color, const dfx_plane* ssr, const dfx_plane* ao, float ssr_scale, float ssao_scale,
                                         const dfx_plane* prev_accum, const dfx_plane* closest_motion, const dfx_plane* reprojected_depth,

@@ -212,6 +212,9 @@ int run_pass_impl(Ctx& c, const std::string& p)
         // Bloom::Execute (Bloom.cpp:407-436)
         const TexF4& in   = c.f4["bloom_in"];
         const int    mips = bloom_mip_count(std::max(in.w / 2, 1), std::max(in.h / 2, 1), c.bloom.Radius);
+        // the composite samples up(0), which only the upsampling of a second level writes: refuse like the CUDA effect does
+        if (mips < 2) return c.err = "Bloom radius " + std::to_string(c.bloom.Radius) + " leaves fewer than two pyramid levels at " +
+                                     std::to_string(in.w) + "x" + std::to_string(in.h), 1;
         auto dn = [&](int i) -> TexF4& { return c.f4["bloom_down" + std::to_string(i)]; };
         auto up = [&](int i) -> TexF4& { return c.f4["bloom_up" + std::to_string(i)]; };
         auto store = [&](TexF4& t) { if (c.faithful) quant(t, F_R11G11B10); }; // every Bloom target is R11G11B10_FLOAT (Bloom.cpp:111, :125, :137)

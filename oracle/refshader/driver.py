@@ -13,7 +13,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from diligentfx_b200 import capi
+from diligentfx_b200 import capi, synth
 from oracle import oracle_py as op
 from oracle.refshader import refsh
 
@@ -36,9 +36,89 @@ class Variant:
     tonemap: capi.ToneMapAttribs = field(default_factory=capi.ToneMapAttribs.default)
     dof_attribs: capi.DOFAttribs = field(default_factory=capi.DOFAttribs.default)
     ave_log_lum: float = 0.3
+    lens: tuple[float, float] | None = None   # (fFocusDistance, fFStop) written into both cameras of every frame; None = synth's
 
     def stages(self) -> int:
         return op.STAGE_ALL | (op.STAGE_DOF if self.dof else 0)
+
+
+EDGE_SIZES = [(8, 8), (17, 5), (33, 17)]   # every pyramid reaches 1 x 1 and the odd-size branches run; 8 x 8 is DoF's minimum
+
+
+def _uniform(rng, lo: float, hi: float) -> float:
+    return float(rng.uniform(lo, hi))
+
+
+def _alpha(rng) -> float:
+    """AlphaInterpolation in (0, 1]: 1 (a settled effect) half of the time."""
+    return 1.0 if rng.random() < 0.5 else float(1.0 - rng.uniform(0.0, 0.95))
+
+
+def random_variant(rng: np.random.Generator, size: tuple[int, int] | None = None) -> tuple[int, int, int, Variant]:
+    """One seeded draw of (width, height, scene seed, Variant): frame size (or `size`), feature flags, tone-map operator and every
+    attribute field the passes read. Shared by the oracle-vs-shader test and the CUDA-vs-oracle tests, so both links are checked
+    at the same configurations. Combinations the reference builds no shader variant for are folded onto ones it does."""
+    w, h = size if size is not None else (int(rng.integers(40, 220)), int(rng.integers(30, 130)))
+    v = Variant(reversed_depth=bool(rng.random() < 0.25), ssr_flags=int(rng.integers(0, 3)), ssao_flags=int(rng.integers(0, 3)),
+                ssao_algorithm=int(rng.integers(0, 3)), taa_flags=int(rng.integers(0, 8)), tonemap_mode=int(rng.integers(1, 12)),
+                to_srgb=bool(rng.integers(0, 2)), dof=bool(rng.integers(0, 2)) and min(w, h) >= 8, dof_flags=int(rng.integers(0, 4)))
+    if v.ssao_algorithm:
+        v.ssao_flags = 0                                  # HBAO / VBAO are built for the full-resolution, full-precision path
+    if v.reversed_depth:                                  # the inverted-depth shaders exist for the default SSR / GTAO path
+        v.ssr_flags = v.ssao_flags = v.ssao_algorithm = 0
+        v.dof = False
+    s = v.ssr
+    s.DepthBufferThickness, s.RoughnessThreshold = _uniform(rng, 0.005, 0.1), _uniform(rng, 0.05, 0.6)
+    s.MostDetailedMip, s.IsRoughnessPerceptual, s.RoughnessChannel = int(rng.integers(0, 3)), int(rng.integers(0, 2)), int(rng.integers(0, 4))
+    s.MaxTraversalIntersections = int(rng.integers(1, 17)) if rng.random() < 0.4 else int(rng.integers(17, 200))
+    s.GGXImportanceSampleBias, s.SpatialReconstructionRadius = _uniform(rng, 0, 1), _uniform(rng, 0, 6)
+    s.TemporalRadianceStabilityFactor, s.TemporalVarianceStabilityFactor = _uniform(rng, 0, 1), _uniform(rng, 0, 1)
+    s.BilateralCleanupSpatialSigmaFactor, s.AlphaInterpolation = _uniform(rng, 0.2, 1.5), _alpha(rng)
+    a = v.ssao
+    a.EffectRadius, a.EffectFalloffRange, a.RadiusMultiplier = _uniform(rng, 0.2, 3), _uniform(rng, 0.1, 1), _uniform(rng, 0.5, 2.5)
+    a.DepthMIPSamplingOffset, a.TemporalStabilityFactor = _uniform(rng, 1, 5), _uniform(rng, 0, 1)
+    a.SpatialReconstructionRadius = _uniform(rng, 0.5, 4.0) if rng.random() < 0.5 else _uniform(rng, 4.0, 8.0)   # both sides of the tile kernel's limit
+    a.AlphaInterpolation, a.BitmaskThickness = _alpha(rng), _uniform(rng, 0.05, 1)
+    b = v.bloom
+    b.Threshold, b.SoftTreshold, b.Intensity, b.Radius = _uniform(rng, 0, 2), _uniform(rng, 0, 1), _uniform(rng, 0, 1), _uniform(rng, 0.5, 1.0)
+    b.AlphaInterpolation = _alpha(rng)
+    levels = lambda: op.lib().orc_bloom_mip_count(max(w // 2, 1), max(h // 2, 1), C.c_float(b.Radius))  # noqa: E731
+    while levels() < 2:                                   # Bloom refuses a pyramid of one level
+        b.Radius = min(1.0, b.Radius + 0.125)
+    v.taa.TemporalStabilityFactor, v.taa.SkipRejection = _uniform(rng, 0, 1), int(rng.integers(0, 2))
+    m = v.tonemap
+    m.bAutoExposure, m.bLightAdaptation = int(rng.integers(0, 2)), int(rng.integers(0, 2))
+    m.fMiddleGray, m.fWhitePoint, m.fLuminanceSaturation = _uniform(rng, 0.05, 0.5), _uniform(rng, 1, 8), _uniform(rng, 0.5, 2)
+    m.AgXSaturation, m.AgXSlope, m.AgXPower, m.AgXOffset = _uniform(rng, 0.5, 1.5), _uniform(rng, 0.7, 1.3), _uniform(rng, 0.7, 1.3), _uniform(rng, -0.05, 0.05)
+    v.ave_log_lum = _uniform(rng, 0.05, 1.5)
+    d = v.dof_attribs
+    d.MaxCircleOfConfusion, d.TemporalStabilityFactor = _uniform(rng, 0.005, 0.03), _uniform(rng, 0, 1)
+    d.BokehKernelRingCount, d.BokehKernelRingDensity, d.AlphaInterpolation = int(rng.integers(2, 6)), int(rng.integers(2, 8)), _alpha(rng)
+    if v.dof:
+        v.lens = (_uniform(rng, 2, 12), _uniform(rng, 1.2, 8))
+    return w, h, int(rng.integers(1, 1000)), v
+
+
+def random_trial(trial: int | str) -> tuple[np.random.Generator, tuple[int, int] | None]:
+    """The generator and size of a test trial: an integer draws a random size, "WxH" (one of EDGE_SIZES) fixes it."""
+    if isinstance(trial, str):
+        w, h = (int(x) for x in trial.split("x"))
+        return np.random.default_rng(4096 + 1000 * w + h), (w, h)
+    return np.random.default_rng(2024 + trial), None
+
+
+def variant_sequence(w: int, h: int, seed: int, v: Variant, frames: int) -> list[dict]:
+    """The synthetic sequence a drawn variant runs on: reversed depth and the lens of `v` applied to every frame."""
+    seq = synth.generate_sequence(w, h, frames, seed=seed)
+    if v.reversed_depth:
+        seq = [synth.reverse_depth_frame(f) for f in seq]
+    if v.lens is not None:
+        for f in seq:
+            for k in ("curr_camera", "prev_camera"):
+                c = capi.CameraAttribs.from_buffer_copy(bytes(f[k]))
+                c.fFocusDistance, c.fFStop = v.lens
+                f[k] = c
+    return seq
 
 
 def make_oracle(width: int, height: int, v: Variant) -> op.Oracle:

@@ -1,0 +1,426 @@
+"""The CUDA counterpart of oracle/refshader/driver.compare_frame: steps the oracle through one frame pass by pass and, beside every
+oracle pass, runs the CUDA pass through the C-ABI on that pass's oracle input planes. A difference is therefore attributable to
+the one pass. Returns {label: (cuda_output, oracle_output)} with compare_frame's labels (P0 ... M1, D1 ... D11) plus the fused
+entries and the Bloom pyramid launch shapes, which have labels of their own.
+
+Every device plane is allocated in one of three layouts:
+  "tight"   pitch = width * bytes per texel (what capi.plane_of describes);
+  "padded"  one or more texels of padding per row, pitch not a multiple of 16 bytes where the texel size allows it (the TMA paths
+            need a 16-byte multiple and fall back to plain loads);
+  "aligned" pitch rounded up to 128 bytes, like dfx_plane_alloc (the TMA paths run).
+The padding is filled with NaN (0xA5 for the 8-bit masks): a kernel that indexes rows with the width where it should use the
+pitch, or that reads past the end of a row, turns up as a NaN or a wrong value; `Planes.padding_damage()` reports writes into it.
+
+Test infrastructure only; it never runs the reference's shaders.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+
+from diligentfx_b200 import capi
+from oracle import oracle_py as op
+from oracle.refshader.driver import Variant, _count, _levels
+
+LAYOUTS = ("tight", "padded", "aligned")
+MASK_FILL = 0xA5
+
+
+class Buf:
+    """One device plane: `storage` is the whole allocation (padding included), `t` the (H, W[, C]) view of its texels."""
+
+    def __init__(self, storage, t, plane: capi.Plane, row_elems: int):
+        self.storage, self.t, self.p, self.row_elems = storage, t, plane, row_elems
+
+    @property
+    def ref(self):
+        return C.byref(self.p)
+
+    def host(self) -> np.ndarray:
+        return self.t.cpu().numpy().astype(np.float32)
+
+
+class Planes:
+    """Allocates device planes in one layout and keeps them (and their descriptors) alive."""
+
+    _FMT = {(torch.float32, 1): (capi.FORMAT_R32F, 4), (torch.float32, 2): (capi.FORMAT_RG32F, 8), (torch.float32, 4): (capi.FORMAT_RGBA32F, 16),
+            (torch.uint8, 1): (capi.FORMAT_R8U, 1)}
+
+    def __init__(self, layout: str = "tight"):
+        assert layout in LAYOUTS, layout
+        self.layout, self.bufs, self.keep = layout, [], []
+
+    def pitch(self, w: int, bpt: int) -> int:
+        if self.layout == "tight":
+            return w * bpt
+        if self.layout == "aligned":
+            return -(-w * bpt // 128) * 128
+        p = w * bpt + bpt
+        while p % 16 == 0 and bpt < 16:                    # RGBA32F texels are 16 bytes: every pitch is a multiple of 16
+            p += bpt
+        return p
+
+    def new(self, h: int, w: int, ch: int = 1, fill: float | np.ndarray | None = None, flags: int = 0, dtype=torch.float32) -> Buf:
+        fmt, bpt = self._FMT[(dtype, ch)]
+        pitch = self.pitch(w, bpt)
+        esz = 1 if dtype == torch.uint8 else 4
+        pad_value = MASK_FILL if dtype == torch.uint8 else float("nan")
+        storage = torch.full((h * pitch // esz,), pad_value, dtype=dtype, device="cuda")
+        row = pitch // esz
+        t = storage.as_strided((h, w) if ch == 1 else (h, w, ch), (row, 1) if ch == 1 else (row, ch, 1))
+        if isinstance(fill, np.ndarray):
+            t.copy_(torch.from_numpy(np.ascontiguousarray(fill, np.uint8 if dtype == torch.uint8 else np.float32)).cuda())
+        elif fill is not None:
+            t.fill_(fill)
+        b = Buf(storage, t, capi.Plane(storage.data_ptr(), pitch, w, h, fmt, flags), row)
+        self.bufs.append(b)
+        return b
+
+    def up(self, a: np.ndarray, flags: int = 0) -> Buf:
+        a = np.asarray(a, np.float32)
+        return self.new(a.shape[0], a.shape[1], 1 if a.ndim == 2 else a.shape[2], fill=a, flags=flags)
+
+    def mask(self, a: np.ndarray) -> Buf:
+        return self.new(a.shape[0], a.shape[1], fill=(np.asarray(a) != 0).astype(np.uint8), dtype=torch.uint8)
+
+    def like(self, a: np.ndarray, fill=None, flags: int = 0) -> Buf:
+        return self.new(a.shape[0], a.shape[1], 1 if a.ndim == 2 else a.shape[2], fill=fill, flags=flags)
+
+    def pyramid(self, bufs: list[Buf]) -> capi.Pyramid:
+        p = capi.Pyramid()
+        p.levels = len(bufs)
+        for i, b in enumerate(bufs):
+            p.level[i] = b.p
+        self.keep.append(p)
+        return p
+
+    def array(self, bufs: list[Buf]):
+        arr = (capi.Plane * len(bufs))(*[b.p for b in bufs])
+        self.keep.append(arr)
+        return arr
+
+    def cameras(self, curr, prev):
+        buf = (capi.CameraAttribs * 2)(curr, prev)
+        t = torch.frombuffer(bytearray(bytes(buf)), dtype=torch.uint8).cuda()
+        self.keep.append(t)
+        return C.c_void_p(t.data_ptr())
+
+    def padding_damage(self) -> int:
+        """Number of planes whose row padding no longer holds the fill value."""
+        bad = 0
+        for b in self.bufs:
+            s = b.storage.cpu().numpy().reshape(b.p.height, b.row_elems)
+            pad = s[:, b.t.shape[1] * (b.t.shape[2] if b.t.dim() == 3 else 1):]
+            if pad.size and not (np.isnan(pad).all() if pad.dtype != np.uint8 else (pad == MASK_FILL).all()):
+                bad += 1
+        return bad
+
+
+def rows(h: int) -> capi.Rows:
+    return capi.Rows(0, h)
+
+
+def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes: Planes | None = None) -> dict[str, tuple[np.ndarray, np.ndarray]]:
+    """`o` holds the history of the frames before `fr` (run with o.frame()); `fr` must be the next frame of the sequence. Outputs
+    that a pass leaves untouched where its mask is off (S2 roughness, S5, S6) are pre-filled with the oracle's contents from
+    before the pass, so they compare bit for bit there. `planes` (optional) receives the allocations for a padding check."""
+    L = capi.load()
+    P = planes if planes is not None else Planes(layout)
+    res: dict[str, tuple[np.ndarray, np.ndarray]] = {}
+    rev = capi.PLANE_FLAG_REVERSED_DEPTH if v.reversed_depth else 0
+    ci, pi = fr["frame"] & 1, (fr["frame"] + 1) & 1
+    o.set_inputs(fr)
+    g = o.get
+    cams = P.cameras(fr["curr_camera"], fr["prev_camera"])
+    H, W = fr["depth"].shape
+
+    def ok(status, what):
+        capi.check(status, what)
+
+    # ---------------- PostFXContext ----------------
+    tables = torch.from_numpy(np.fromfile(op.TABLES, np.uint8)).cuda()
+    P.keep.append(tables)
+    xy, zw = P.new(128, 128, 2), P.new(128, 128, 2)
+    ok(L.dfx_pass_blue_noise(None, C.c_void_p(tables.data_ptr()), fr["frame"], xy.ref, zw.ref), "blue noise")
+    o.run("blue_noise")
+    res["P0 blue_noise.xy"], res["P0 blue_noise.zw"] = (xy.host(), g("bn_xy")), (zw.host(), g("bn_zw"))
+    depth_np, motion_np, normal_np, color_np, material_np = g("depth"), g("motion"), g("normal"), g("color"), g("material")
+    depth, motion, normal, color, material = P.up(depth_np, rev), P.up(motion_np), P.up(normal_np), P.up(color_np), P.up(material_np)
+    rp, cm, pd = P.new(H, W, flags=rev), P.new(H, W, 2), P.new(H, W, flags=rev)
+    ok(L.dfx_pass_postfx_prepare(None, cams, depth.ref, P.up(g("prev_depth_in"), rev).ref, motion.ref, rp.ref, cm.ref, pd.ref, rows(H)), "postfx prepare")
+    o.run("reprojected_depth"), o.run("closest_motion"), o.run("previous_depth")
+    reproj_np, closest_np, prev_depth_np = g("reproj_depth"), g("closest_motion"), g("prev_depth")
+    res["P1 reprojected_depth"], res["P2 closest_motion"], res["P3 previous_depth"] = (rp.host(), reproj_np), (cm.host(), closest_np), (pd.host(), prev_depth_np)
+    reproj, closest, prev_depth = P.up(reproj_np, rev), P.up(closest_np), P.up(prev_depth_np, rev)
+
+    # ---------------- ScreenSpaceReflection ----------------
+    A = v.ssr
+    half = bool(v.ssr_flags & capi.SSR_FLAG_HALF_RESOLUTION)
+    o.run("ssr_hiz")
+    hiz = _levels(o, "ssr_hiz")
+    lv = [depth] + [P.like(m) for m in hiz[1:]]
+    ok(L.dfx_pass_ssr_hiz(None, C.byref(P.pyramid(lv)), rows(H)), "ssr hiz")
+    for i in range(1, len(hiz)):
+        res[f"S1 ssr_hiz.{i}"] = (lv[i].host(), hiz[i])
+    hiz_pyr = P.pyramid([depth] + [P.up(m) for m in hiz[1:]])
+    rough_before = g("ssr_roughness")
+    o.run("ssr_mask")
+    rough_np, maskf = g("ssr_roughness"), g("ssr_mask")
+    r_out, m_out = P.up(rough_before), P.new(H, W, fill=7, dtype=torch.uint8)
+    ok(L.dfx_pass_ssr_mask_roughness(None, C.byref(A), material.ref, depth.ref, r_out.ref, m_out.ref, rows(H)), "ssr mask")
+    res["S2 ssr_roughness"], res["S2 ssr_stencil"] = (r_out.host(), rough_np), (m_out.host(), maskf)
+    rough, mask = P.up(rough_np), P.mask(maskf)
+    trace_mask = mask
+    if half:
+        o.run("ssr_downsample_mask")
+        mh = g("ssr_mask_half")
+        out = P.new(mh.shape[0], mh.shape[1], fill=7, dtype=torch.uint8)
+        ok(L.dfx_pass_ssr_downsample_mask(None, C.byref(A), rough.ref, depth.ref, out.ref, rows(mh.shape[0])), "ssr downsample mask")
+        res["S3 ssr_stencil_half"] = (out.host(), mh)
+        trace_mask = P.mask(mh)
+    o.run("ssr_intersect")
+    rad_np, rdir_np = g("ssr_radiance"), g("ssr_raydir")
+    rad, rdir = P.like(rad_np, fill=-1.0), P.like(rdir_np, fill=-1.0)
+    bn_xy = P.up(g("bn_xy"))
+    ok(L.dfx_pass_ssr_intersect(None, cams, C.byref(A), v.ssr_flags, color.ref, normal.ref, rough.ref, trace_mask.ref, bn_xy.ref, C.byref(hiz_pyr),
+                                motion.ref, rad.ref, rdir.ref, rows(rad_np.shape[0])), "ssr intersect")
+    res["S4 ssr_intersect.radiance"], res["S4 ssr_intersect.raydir_pdf"] = (rad.host(), rad_np), (rdir.host(), rdir_np)
+    pre = [g("ssr_resolved_rad"), g("ssr_resolved_var"), g("ssr_resolved_depth")]
+    o.run("ssr_spatial")
+    want = [g("ssr_resolved_rad"), g("ssr_resolved_var"), g("ssr_resolved_depth")]
+    outs = [P.up(p) for p in pre]
+    ok(L.dfx_pass_ssr_spatial(None, cams, C.byref(A), rough.ref, mask.ref, normal.ref, depth.ref, P.up(rdir_np).ref, P.up(rad_np).ref,
+                              *[b.ref for b in outs], rows(H)), "ssr spatial")
+    for n_, b_, w_ in zip(("radiance", "variance", "depth"), outs, want):
+        res[f"S5 ssr_spatial.{n_}"] = (b_.host(), w_)
+    pre = [g(f"ssr_radhist{ci}"), g(f"ssr_varhist{ci}")]
+    ins = [motion, P.up(want[2]), reproj, P.up(want[0]), P.up(want[1]), prev_depth, P.up(g(f"ssr_radhist{pi}")), P.up(g(f"ssr_varhist{pi}"))]
+    o.run("ssr_temporal")
+    acc = [g(f"ssr_radhist{ci}"), g(f"ssr_varhist{ci}")]
+    outs = [P.up(p) for p in pre]
+    ok(L.dfx_pass_ssr_temporal(None, cams, C.byref(A), mask.ref, *[b.ref for b in ins], *[b.ref for b in outs], rows(H)), "ssr temporal")
+    res["S6 ssr_temporal.radiance"], res["S6 ssr_temporal.variance"] = (outs[0].host(), acc[0]), (outs[1].host(), acc[1])
+    o.run("ssr_bilateral")
+    ssr_out_np = g("ssr_out")
+    out = P.like(ssr_out_np, fill=5.0)
+    ok(L.dfx_pass_ssr_bilateral(None, cams, C.byref(A), mask.ref, depth.ref, normal.ref, rough.ref, P.up(acc[0]).ref, P.up(acc[1]).ref, out.ref, rows(H)), "ssr bilateral")
+    res["S7 ssr_bilateral"] = (out.host(), ssr_out_np)
+
+    # ---------------- ScreenSpaceAmbientOcclusion ----------------
+    S = v.ssao
+    S.Algorithm = v.ssao_algorithm
+    ao_half = bool(v.ssao_flags & capi.SSAO_FLAG_HALF_RESOLUTION)
+    src_flags = rev | (2 if v.ssao_flags & 1 else 0)                          # DFX_PLANE_FLAG_HALF_PRECISION_DEPTH
+    src = depth_np
+    if ao_half:
+        o.run("ssao_downsample")
+        src = g("ssao_checker")
+        out = P.like(src, fill=-3.0)
+        ok(L.dfx_pass_ssao_downsample_depth(None, depth.ref, out.ref, rows(src.shape[0])), "ssao downsample")
+        res["A0 ssao_downsample"] = (out.host(), src)
+    o.run("ssao_prefilter")
+    pre = _levels(o, "ssao_pre")
+    lv = [P.up(src, src_flags)] + [P.like(m, fill=-3.0) for m in pre[1:]]
+    ok(L.dfx_pass_ssao_prefilter_depth(None, cams, C.byref(S), C.byref(P.pyramid(lv)), rows(src.shape[0])), "ssao prefilter")
+    for i in range(1, len(pre)):
+        res[f"A1 ssao_prefilter.{i}"] = (lv[i].host(), pre[i])
+    o.run("ssao_ao")
+    occ_np = g("ssao_occ")
+    out = P.like(occ_np, fill=-3.0)
+    pyr = P.pyramid([P.up(pre[0], src_flags)] + [P.up(m) for m in pre[1:]])
+    ok(L.dfx_pass_ssao_ambient_occlusion(None, cams, C.byref(S), C.byref(pyr), normal.ref, P.up(g("bn_zw")).ref, out.ref, rows(occ_np.shape[0])), "ssao ao")
+    res["A2 ssao_ao"] = (out.host(), occ_np)
+    if ao_half:
+        o.run("ssao_upsample")
+        up_np = g("ssao_occ_up")
+        out = P.like(up_np, fill=-3.0)
+        ok(L.dfx_pass_ssao_upsample(None, cams, depth.ref, P.up(occ_np).ref, out.ref, rows(H)), "ssao upsample")
+        res["A4 ssao_upsample"] = (out.host(), up_np)
+        occ_np = up_np
+    ins = [P.up(occ_np), P.up(g(f"ssao_hist{pi}")), P.up(g(f"ssao_histlen{pi}")), reproj, prev_depth, closest]
+    o.run("ssao_temporal")
+    acc_o, hlen = g("ssao_acc"), g(f"ssao_histlen{ci}")
+    oo, oh = P.new(H, W, fill=-3.0), P.new(H, W, fill=-3.0)
+    ok(L.dfx_pass_ssao_temporal(None, cams, C.byref(S), *[b.ref for b in ins], oo.ref, oh.ref, rows(H)), "ssao temporal")
+    res["A5 ssao_temporal.occlusion"], res["A5 ssao_temporal.history"] = (oo.host(), acc_o), (oh.host(), hlen)
+    o.run("ssao_convolute")
+    co, cd = _levels(o, "ssao_conv_occ"), _levels(o, "ssao_conv_depth")
+    lo = [P.up(co[0])] + [P.like(m, fill=-3.0) for m in co[1:]]
+    ld = [depth] + [P.like(m, fill=-3.0) for m in cd[1:]]
+    ok(L.dfx_pass_ssao_convolute(None, C.byref(P.pyramid(lo)), C.byref(P.pyramid(ld)), rows(H)), "ssao convolute")
+    for i in range(1, len(co)):
+        res[f"A6 ssao_convolute.occlusion.{i}"], res[f"A6 ssao_convolute.depth.{i}"] = (lo[i].host(), co[i]), (ld[i].host(), cd[i])
+    o.run("ssao_resample")
+    rs = g("ssao_resampled")
+    hl = P.up(hlen)
+    out = P.new(H, W, fill=-3.0)
+    po, pdp = P.pyramid([P.up(m) for m in co]), P.pyramid([depth] + [P.up(m) for m in cd[1:]])
+    ok(L.dfx_pass_ssao_resample(None, cams, C.byref(po), C.byref(pdp), hl.ref, normal.ref, out.ref, rows(H)), "ssao resample")
+    res["A7 ssao_resample"] = (out.host(), rs)
+    o.run("ssao_spatial")
+    ao_np = g("ssao_out")
+    out = P.new(H, W, fill=-3.0)
+    ok(L.dfx_pass_ssao_spatial(None, cams, C.byref(S), P.up(rs).ref, hl.ref, depth.ref, normal.ref, out.ref, rows(H)), "ssao spatial")
+    res["A8 ssao_spatial"] = (out.host(), ao_np)
+
+    # ---------------- compose -> TAA (separate and fused) ----------------
+    ssr_out, ao = P.up(ssr_out_np), P.up(ao_np)
+    scales = (C.c_float(1.0), C.c_float(1.0))                                 # the oracle's compose scales (orc_create)
+    o.run("compose")
+    composed = g("composed")
+    out = P.like(composed, fill=-3.0)
+    ok(L.dfx_pass_compose(None, color.ref, ssr_out.ref, ao.ref, *scales, out.ref, rows(H)), "compose")
+    res["C1 compose"] = (out.host(), composed)
+    o.set("taa_in", composed)
+    v.taa.ResetAccumulation = 0                                               # consecutive frame (TemporalAntiAliasing.cpp:125-128)
+    o.set_taa(v.taa, v.taa_flags)
+    prev_acc = g(f"taa_accum{pi}")
+    o.run("taa")
+    acc_t = g(f"taa_accum{ci}")
+    taa_ins = [P.up(prev_acc), closest, reproj, prev_depth]
+    out = P.like(acc_t, fill=-3.0)
+    ok(L.dfx_pass_taa(None, cams, C.byref(v.taa), v.taa_flags, P.up(composed).ref, *[b.ref for b in taa_ins], out.ref, rows(H)), "taa")
+    res["T1 taa"] = (out.host(), acc_t)
+    out = P.like(acc_t, fill=-3.0)
+    ok(L.dfx_pass_compose_taa(None, cams, C.byref(v.taa), v.taa_flags, color.ref, ssr_out.ref, ao.ref, *scales, *[b.ref for b in taa_ins], out.ref, rows(H)),
+       "compose + taa")
+    res["T1 compose_taa (fused)"] = (out.host(), acc_t)
+    post_in = acc_t
+
+    # ---------------- DepthOfField ----------------
+    if v.dof:
+        a, f = v.dof_attribs, v.dof_flags
+        o.set("dof_in", post_in)
+        pin = P.up(post_in)
+        o.run("dof_coc")
+        coc = g("dof_coc")
+        out = P.like(coc, fill=-3.0)
+        ok(L.dfx_pass_dof_coc(None, cams, C.byref(a), depth.ref, out.ref, rows(H)), "dof coc")
+        res["D1 dof_coc"] = (out.host(), coc)
+        if f & capi.DOF_FLAG_TEMPORAL_SMOOTHING:
+            prevc = g(f"dof_coc_temporal{pi}")
+            o.run("dof_temporal")
+            tc = g(f"dof_coc_temporal{ci}")
+            out = P.like(tc, fill=-3.0)
+            ok(L.dfx_pass_dof_temporal_coc(None, cams, C.byref(a), P.up(coc).ref, P.up(prevc).ref, closest.ref, out.ref, rows(H)), "dof temporal")
+            res["D2 dof_temporal"] = (out.host(), tc)
+            coc = tc
+        cb = P.up(coc)
+        o.run("dof_separated")
+        d0 = g("dof_dilation0")
+        out = P.like(d0, fill=-3.0)
+        ok(L.dfx_pass_dof_separated_coc(None, cb.ref, out.ref, rows(H)), "dof separated")
+        res["D3 dof_separated"] = (out.host(), d0)
+        o.run("dof_dilation")
+        dl = [g(f"dof_dilation{i}") for i in range(4)]
+        for i in range(3):
+            out = P.like(dl[i + 1], fill=-3.0)
+            ok(L.dfx_pass_dof_dilation(None, P.up(dl[i]).ref, out.ref, rows(dl[i + 1].shape[0])), "dof dilation")
+            res[f"D4 dof_dilation.{i + 1}"] = (out.host(), dl[i + 1])
+        o.run("dof_blur_x")
+        bx = g("dof_dilation_tmp")
+        out = P.like(bx, fill=-3.0)
+        ok(L.dfx_pass_dof_blur_coc(None, P.up(dl[3]).ref, 0, out.ref, rows(bx.shape[0])), "dof blur x")
+        res["D5 dof_blur_x"] = (out.host(), bx)
+        o.run("dof_blur_y")
+        by = g("dof_dilation3")
+        out = P.like(by, fill=-3.0)
+        ok(L.dfx_pass_dof_blur_coc(None, P.up(bx).ref, 1, out.ref, rows(by.shape[0])), "dof blur y")
+        res["D6 dof_blur_y"] = (out.host(), by)
+        o.run("dof_prefilter")
+        p0, p1 = g("dof_pre0"), g("dof_pre1")
+        o0, o1 = P.like(p0, fill=-3.0), P.like(p1, fill=-3.0)
+        ok(L.dfx_pass_dof_prefilter(None, pin.ref, cb.ref, P.up(by).ref, o0.ref, o1.ref, rows(p0.shape[0])), "dof prefilter")
+        res["D7 dof_prefilter.near"], res["D7 dof_prefilter.far"] = (o0.host(), p0), (o1.host(), p1)
+        o.run("dof_bokeh_first")
+        b0, b1 = g("dof_bokeh0"), g("dof_bokeh1")
+        o0, o1 = P.like(b0, fill=-3.0), P.like(b1, fill=-3.0)
+        ok(L.dfx_pass_dof_bokeh(None, cams, C.byref(a), f, 0, P.up(p0).ref, P.up(p1).ref, pin.ref, o0.ref, o1.ref, rows(b0.shape[0])), "dof bokeh 1")
+        res["D8 dof_bokeh_first.near"], res["D8 dof_bokeh_first.far"] = (o0.host(), b0), (o1.host(), b1)
+        o.run("dof_bokeh_second")
+        s0, s1 = g("dof_pre0"), g("dof_pre1")
+        o0, o1 = P.like(s0, fill=-3.0), P.like(s1, fill=-3.0)
+        ok(L.dfx_pass_dof_bokeh(None, cams, C.byref(a), f, 1, P.up(b0).ref, P.up(b1).ref, None, o0.ref, o1.ref, rows(s0.shape[0])), "dof bokeh 2")
+        res["D9 dof_bokeh_second.near"], res["D9 dof_bokeh_second.far"] = (o0.host(), s0), (o1.host(), s1)
+        o.run("dof_postfilter")
+        f0, f1 = g("dof_bokeh0"), g("dof_bokeh1")
+        o0, o1 = P.like(f0, fill=-3.0), P.like(f1, fill=-3.0)
+        ok(L.dfx_pass_dof_postfilter(None, P.up(s0).ref, P.up(s1).ref, o0.ref, o1.ref, rows(f0.shape[0])), "dof postfilter")
+        res["D10 dof_postfilter.near"], res["D10 dof_postfilter.far"] = (o0.host(), f0), (o1.host(), f1)
+        o.run("dof_combine")
+        dout = g("dof_out")
+        out = P.like(dout, fill=-3.0)
+        ok(L.dfx_pass_dof_combine(None, C.byref(a), pin.ref, P.up(f0).ref, P.up(f1).ref, out.ref, rows(H)), "dof combine")
+        res["D11 dof_combine"] = (out.host()[..., :3], dout[..., :3])
+        post_in = dout
+
+    # ---------------- Bloom (RGB compared: alpha is not part of the reference's R11G11B10 chain) ----------------
+    B = v.bloom
+    o.set("bloom_in", post_in)
+    o.run("bloom")
+    n = _count(o, "bloom_down")
+    dn, up = [g(f"bloom_down{i}") for i in range(n)], [g(f"bloom_up{i}") for i in range(n - 1)]
+    pin = P.up(post_in)
+    out = P.like(dn[0], fill=-3.0)
+    ok(L.dfx_pass_bloom_prefilter(None, C.byref(B), pin.ref, out.ref, rows(dn[0].shape[0])), "bloom prefilter")
+    res["B1 bloom_prefilter"] = (out.host()[..., :3], dn[0][..., :3])
+    dn_dev = [P.up(m) for m in dn]
+    for i in range(1, n):
+        out = P.like(dn[i], fill=-3.0)
+        ok(L.dfx_pass_bloom_downsample(None, dn_dev[i - 1].ref, out.ref, rows(dn[i].shape[0])), "bloom downsample")
+        res[f"B2 bloom_downsample.{i}"] = (out.host()[..., :3], dn[i][..., :3])
+    top = n - 1
+    for i in range(top, 0, -1):
+        out = P.like(up[i - 1], fill=-3.0)
+        coarser = P.up(up[i]) if i != top else dn_dev[i]
+        ok(L.dfx_pass_bloom_upsample(None, dn_dev[i - 1].ref, coarser.ref, out.ref, rows(up[i - 1].shape[0])), "bloom upsample")
+        res[f"B3 bloom_upsample.{i - 1}"] = (out.host()[..., :3], up[i - 1][..., :3])
+    # the two pyramid launch shapes: every level after the first in one thread-block cluster (tail) / one cooperative grid (levels)
+    for shape in ("tail", "levels"):
+        dn_o, up_o = [dn_dev[0]] + [P.like(m, fill=-3.0) for m in dn[1:]], [P.like(m, fill=-3.0) for m in dn]
+        pd_, pu_ = P.array(dn_o), P.array(up_o)
+        if shape == "tail":
+            L.dfx_tune_set(b"bloom_tail", 1), L.dfx_tune_set(b"bloom_tail_texels", 1 << 30)
+            try:
+                first = L.dfx_bloom_tail_first_level(pd_, n)
+            finally:
+                L.dfx_tune_unset(b"bloom_tail"), L.dfx_tune_unset(b"bloom_tail_texels")
+            assert first == 1, first
+            ok(L.dfx_pass_bloom_tail(None, pd_, pu_, 1, n), "bloom tail")
+        else:
+            ws = torch.zeros(16, dtype=torch.int32, device="cuda")
+            P.keep.append(ws)
+            ok(L.dfx_pass_bloom_levels(None, pd_, pu_, 1, n, C.c_void_p(ws.data_ptr())), "bloom levels")
+            timed_out = C.c_int32(-1)
+            ok(L.dfx_bloom_levels_check(C.c_void_p(ws.data_ptr()), C.byref(timed_out)), "bloom levels check")
+            assert timed_out.value == 0
+        for i in range(1, n):
+            res[f"B2 bloom_{shape}.down.{i}"] = (dn_o[i].host()[..., :3], dn[i][..., :3])
+        for i in range(n - 1):
+            res[f"B3 bloom_{shape}.up.{i}"] = (up_o[i].host()[..., :3], up[i][..., :3])
+    bout = g("bloom_out")
+    up0 = P.up(up[0])
+    out = P.like(bout, fill=-3.0)
+    ok(L.dfx_pass_bloom_composite(None, C.byref(B), pin.ref, up0.ref, out.ref, rows(H)), "bloom composite")
+    res["B4 bloom_composite"] = (out.host()[..., :3], bout[..., :3])
+
+    # ---------------- ToneMapping + sRGB (separate and fused with the Bloom composite) ----------------
+    T = v.tonemap
+    T.iToneMappingMode = v.tonemap_mode
+    o.set("tonemap_in", bout)
+    o.run("tonemap")
+    ldr = g("ldr")
+    out = P.like(ldr, fill=-3.0)
+    ok(L.dfx_pass_tonemap(None, C.byref(T), C.c_float(v.ave_log_lum), int(v.to_srgb), P.up(bout).ref, out.ref, rows(H)), "tonemap")
+    res["M1 tonemap"] = (out.host(), ldr)
+    out = P.like(ldr, fill=-3.0)
+    st = L.dfx_pass_bloom_composite_tonemap(None, C.byref(B), C.byref(T), C.c_float(v.ave_log_lum), int(v.to_srgb), pin.ref, up0.ref, out.ref, rows(H))
+    if up[0].shape[0] * 2 == H and up[0].shape[1] * 2 == W:
+        ok(st, "bloom composite + tonemap")
+        res["M1 bloom_composite_tonemap (fused)"] = (out.host(), ldr)
+    else:                                                                     # odd frame size: no exact 2:1 level, the caller runs B4 and M1
+        assert st == capi.DFX_ERR_UNSUPPORTED, st
+    torch.cuda.synchronize()
+    return res

@@ -10,7 +10,6 @@ from diligentfx_b200 import capi, synth
 
 ROOT = capi.REPO_ROOT
 INC = os.path.join(ROOT, "include")
-OUT = os.path.join(ROOT, "tests", "cpp", "_build")
 
 
 @pytest.mark.parametrize("header", ["dfx/DiligentShim.hpp", "dfx/GBuffer.hpp", "dfx/PostFXContext.hpp", "dfx/PostProcessEffects.hpp", "dfx_b200.h"])
@@ -20,9 +19,9 @@ def test_header_is_self_contained(header):
     assert r.returncode == 0, r.stderr.decode()
 
 
-def build_driver(built) -> str:
-    os.makedirs(OUT, exist_ok=True)
-    exe = os.path.join(OUT, "chain_driver")
+def build_driver(built, out_dir) -> str:
+    """Compiles tests/cpp/chain_driver.cpp into `out_dir` (a per-test temporary directory: the repository tree may be read-only)."""
+    exe = os.path.join(str(out_dir), "chain_driver")
     libdir = os.path.dirname(capi.LIB_PATH)
     cmd = ["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", os.path.join(ROOT, "tests", "cpp", "chain_driver.cpp"), "-I", INC, "-L", libdir, "-ldfx_b200",
            f"-Wl,-rpath,{libdir}", "-Wl,--allow-shlib-undefined", "-o", exe]
@@ -31,8 +30,8 @@ def build_driver(built) -> str:
     return exe
 
 
-def test_driver_links_against_the_c_abi_only(built):
-    exe = build_driver(built)
+def test_driver_links_against_the_c_abi_only(built, tmp_path):
+    exe = build_driver(built, tmp_path)
     needed = subprocess.check_output(["objdump", "-p", exe]).decode()
     assert "libdfx_b200.so" in needed
     assert "libcudart" not in "".join(l for l in needed.splitlines() if "NEEDED" in l), "user code must not need CUDA itself"
@@ -41,7 +40,7 @@ def test_driver_links_against_the_c_abi_only(built):
 @pytest.mark.gpu
 def test_cpp_chain_matches_oracle(built, tmp_path):
     from oracle import oracle_py as op
-    exe = build_driver(built)
+    exe = build_driver(built, tmp_path)
     w, h, n = 288, 162, 3
     seq = synth.generate_sequence(w, h, n)
     o = op.Oracle(w, h)
