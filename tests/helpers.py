@@ -1,7 +1,6 @@
-"""Shared helpers for the parity tests: device plane plumbing over the pass-level C-ABI and error metrics."""
+"""Shared helpers for the parity tests: error metrics (device planes: gpu_frame.Planes)."""
 from __future__ import annotations
 
-import ctypes as C
 import os
 import sys
 
@@ -10,8 +9,6 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
-
-from diligentfx_b200 import capi  # noqa: E402
 
 
 def psnr(a: np.ndarray, b: np.ndarray, peak: float = 1.0) -> float:
@@ -51,60 +48,3 @@ def assert_close(name: str, got: np.ndarray, want: np.ndarray, *, tol: float, ma
     if min_psnr is not None:
         assert p >= min_psnr, msg
     return msg
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# device plumbing
-# ---------------------------------------------------------------------------------------------------------------------
-class Dev:
-    """Keeps torch tensors alive while their dfx_plane descriptors are in flight."""
-
-    def __init__(self):
-        import torch
-        self.torch = torch
-        self.lib = capi.load()
-        self.keep = []
-
-    def up(self, a: np.ndarray, dtype=None):
-        t = self.torch.from_numpy(np.ascontiguousarray(a, np.float32 if dtype is None else dtype)).cuda()
-        self.keep.append(t)
-        return t
-
-    def mask(self, a: np.ndarray):
-        t = self.torch.from_numpy(np.ascontiguousarray(a != 0, np.uint8)).cuda()
-        self.keep.append(t)
-        return t
-
-    def empty(self, h: int, w: int, ch: int = 1, fill: float | None = None, dtype=None):
-        shape = (h, w) if ch == 1 else (h, w, ch)
-        dt = dtype or self.torch.float32
-        t = self.torch.empty(shape, dtype=dt, device="cuda") if fill is None else self.torch.full(shape, fill, dtype=dt, device="cuda")
-        self.keep.append(t)
-        return t
-
-    def plane(self, t) -> capi.Plane:
-        p = capi.plane_of(t)
-        self.keep.append(p)
-        return p
-
-    def pyr(self, tensors) -> capi.Pyramid:
-        p = capi.pyramid_of(tensors)
-        self.keep.append(p)
-        return p
-
-    def cameras(self, curr, prev):
-        buf = (capi.CameraAttribs * 2)(curr, prev)
-        t = self.torch.frombuffer(bytearray(bytes(buf)), dtype=self.torch.uint8).cuda()
-        self.keep.append(t)
-        return C.c_void_p(t.data_ptr())
-
-    def sync(self):
-        self.torch.cuda.synchronize()
-
-    @staticmethod
-    def host(t) -> np.ndarray:
-        return t.detach().cpu().numpy().astype(np.float32)
-
-
-def rows(h: int) -> capi.Rows:
-    return capi.Rows(0, h)

@@ -8,8 +8,9 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from helpers import Dev, assert_close, rows
 from diligentfx_b200 import capi, synth
+from gpu_frame import Planes
+from helpers import assert_close
 
 W, H = 96, 54
 
@@ -84,25 +85,22 @@ def test_cuda_brdf_table_and_compose(built):
         o.set(k, v)
     o.set_compose_scales(0.8, 0.6)
     o.run("compose_ibl")
-    d = Dev()
-    lut = d.empty(64, 64, 2, fill=-1.0)
-    capi.check(d.lib.dfx_pass_precompute_brdf_lut(None, 512, C.byref(d.plane(lut))), "brdf lut")
-    d.sync()
+    L, Pl = capi.load(), Planes("tight")
+    lut = Pl.new(64, 64, 2, fill=-1.0)
+    capi.check(L.dfx_pass_precompute_brdf_lut(None, 512, lut.ref), "brdf lut")
     # 512 sequential fp32 additions of sin / cos / pow terms: libm (oracle) and CUDA differ in the last bits of each term
-    assert_close("BRDF table", d.host(lut), o.get("brdf_lut"), tol=3e-4, min_psnr=100.0)
-    cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
-    out = d.empty(H, W, 4, fill=-1.0)
-    P = lambda a: C.byref(d.plane(d.up(a)))  # noqa: E731
-    capi.check(d.lib.dfx_pass_compose_ibl(None, cams, P(p["color"]), P(p["ssr_out"]), P(p["ssao_out"]), P(p["specular_ibl"]), P(p["normal"]),
-                                          P(p["base_color"]), P(p["material"]), P(o.get("brdf_lut")), C.c_float(0.8), C.c_float(0.6),
-                                          C.byref(d.plane(out)), rows(H)), "compose_ibl")
-    d.sync()
-    assert_close("composed (IBL form)", d.host(out), o.get("composed"), tol=1e-4, max_outliers=1e-4, min_psnr=90.0, hdr=True)
+    assert_close("BRDF table", lut.host(), o.get("brdf_lut"), tol=3e-4, min_psnr=100.0)
+    cams = Pl.cameras(fr["curr_camera"], fr["prev_camera"])
+    out = Pl.new(H, W, 4, fill=-1.0)
+    P = lambda a: Pl.up(a).ref  # noqa: E731
+    rows = capi.Rows(0, H)
+    capi.check(L.dfx_pass_compose_ibl(None, cams, P(p["color"]), P(p["ssr_out"]), P(p["ssao_out"]), P(p["specular_ibl"]), P(p["normal"]),
+                                      P(p["base_color"]), P(p["material"]), P(o.get("brdf_lut")), C.c_float(0.8), C.c_float(0.6), out.ref, rows), "compose_ibl")
+    assert_close("composed (IBL form)", out.host(), o.get("composed"), tol=1e-4, max_outliers=1e-4, min_psnr=90.0, hdr=True)
     # without SSR the five extra planes may be null; without AO too -> copy
-    capi.check(d.lib.dfx_pass_compose_ibl(None, cams, P(p["color"]), None, None, None, None, None, None, None, C.c_float(1.0), C.c_float(1.0),
-                                          C.byref(d.plane(out)), rows(H)), "compose_ibl (no SSR, no AO)")
-    d.sync()
-    assert np.array_equal(d.host(out), p["color"])
+    capi.check(L.dfx_pass_compose_ibl(None, cams, P(p["color"]), None, None, None, None, None, None, None, C.c_float(1.0), C.c_float(1.0), out.ref, rows),
+               "compose_ibl (no SSR, no AO)")
+    assert np.array_equal(out.host(), p["color"])
     # SSR given but a plane it needs missing: refused
-    assert d.lib.dfx_pass_compose_ibl(None, cams, P(p["color"]), P(p["ssr_out"]), None, None, P(p["normal"]), P(p["base_color"]), P(p["material"]),
-                                      P(o.get("brdf_lut")), C.c_float(1.0), C.c_float(1.0), C.byref(d.plane(out)), rows(H)) == capi.DFX_ERR_INVALID_ARG
+    assert L.dfx_pass_compose_ibl(None, cams, P(p["color"]), P(p["ssr_out"]), None, None, P(p["normal"]), P(p["base_color"]), P(p["material"]),
+                                  P(o.get("brdf_lut")), C.c_float(1.0), C.c_float(1.0), out.ref, rows) == capi.DFX_ERR_INVALID_ARG

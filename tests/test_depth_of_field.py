@@ -9,8 +9,10 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from helpers import Dev, assert_close, psnr, reinhard, rows
 from diligentfx_b200 import capi, synth
+from gpu_frame import Planes, assert_default, run_sequence
+from helpers import psnr, reinhard
+from oracle.refshader.driver import Variant
 
 W, H, FRAMES = 160, 96, 3
 FLAGS = capi.DOF_FLAG_TEMPORAL_SMOOTHING | capi.DOF_FLAG_KARIS_INVERSE
@@ -98,61 +100,34 @@ def test_oracle_frame_structure(ref):
 
 
 @pytest.mark.gpu
-def test_cuda_dof_passes(ref):
-    seq, o = ref
+def test_cuda_dof_passes(built):
+    """D1 .. D11 against the oracle on its own inputs (gpu_frame.run_frame), then D4 (level 3) -> D5 -> D6 and D7 -> D8 -> D9 -> D10
+    -> D11 on the GPU's own planes against the planes the oracle holds at the end of its frame, all to the default bounds of
+    gpu_frame.tolerance; the D6 blur in place is refused."""
+    v = Variant(dof=True, dof_flags=FLAGS, dof_attribs=_attribs())
+    seq = [_lens(f) for f in synth.generate_sequence(W, H, FRAMES)]
     fr = seq[-1]
-    cur, prv = fr["frame"] & 1, (fr["frame"] + 1) & 1
-    d, a = Dev(), _attribs()
-    L = d.lib
-    cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
-    P = lambda arr: C.byref(d.plane(d.up(arr)))  # noqa: E731
-    hw, hh = W // 2, H // 2
-    # D1
-    coc = d.empty(H, W)
-    capi.check(L.dfx_pass_dof_coc(None, cams, C.byref(a), P(fr["depth"]), C.byref(d.plane(coc)), rows(H)), "D1")
-    assert_close("coc", d.host(coc), o.get("dof_coc"), tol=2e-5)
-    # D2 on the oracle's planes (previous slot = history of frame - 1)
-    tc = d.empty(H, W)
-    capi.check(L.dfx_pass_dof_temporal_coc(None, cams, C.byref(a), P(o.get("dof_coc")), P(o.get(f"dof_coc_temporal{prv}")), P(o.get("closest_motion")),
-                                           C.byref(d.plane(tc)), rows(H)), "D2")
-    assert_close("temporal coc", d.host(tc), o.get(f"dof_coc_temporal{cur}"), tol=2e-5, max_outliers=1e-3)
-    # D3, D4 x3: selections, bit-exact
-    s0 = d.empty(H, W)
-    capi.check(L.dfx_pass_dof_separated_coc(None, P(o.get(f"dof_coc_temporal{cur}")), C.byref(d.plane(s0)), rows(H)), "D3")
-    d.sync()
-    assert np.array_equal(d.host(s0), o.get("dof_dilation0"))
-    for k in range(1, 3):                                      # level 3 is overwritten by the blur in the oracle's frame: check 1 and 2
-        src = o.get(f"dof_dilation{k - 1}")
-        out = d.empty(src.shape[0] >> 1, src.shape[1] >> 1)
-        capi.check(L.dfx_pass_dof_dilation(None, P(src), C.byref(d.plane(out)), rows(out.shape[0])), "D4")
-        d.sync()
-        assert np.array_equal(d.host(out), o.get(f"dof_dilation{k}")), k
-    # D4 (level 3) + D5 + D6 chained, against the blurred level 3
-    l3, tmp = d.empty(H >> 3, W >> 3), d.empty(H >> 3, W >> 3)
-    capi.check(L.dfx_pass_dof_dilation(None, P(o.get("dof_dilation2")), C.byref(d.plane(l3)), rows(H >> 3)), "D4.3")
-    capi.check(L.dfx_pass_dof_blur_coc(None, C.byref(d.plane(l3)), 0, C.byref(d.plane(tmp)), rows(H >> 3)), "D5")
-    capi.check(L.dfx_pass_dof_blur_coc(None, C.byref(d.plane(tmp)), 1, C.byref(d.plane(l3)), rows(H >> 3)), "D6")
-    assert_close("blurred dilation", d.host(l3), o.get("dof_dilation3"), tol=1e-6)
-    assert L.dfx_pass_dof_blur_coc(None, C.byref(d.plane(l3)), 1, C.byref(d.plane(l3)), rows(H >> 3)) == capi.DFX_ERR_INVALID_ARG  # not in-place
-    # D7
-    coc_t = o.get(f"dof_coc_temporal{cur}")
-    fg, bg = d.empty(hh, hw, 4), d.empty(hh, hw, 4)
-    capi.check(L.dfx_pass_dof_prefilter(None, P(o.get("dof_in")), P(coc_t), P(o.get("dof_dilation3")), C.byref(d.plane(fg)), C.byref(d.plane(bg)), rows(hh)), "D7")
-    # the oracle's dof_pre* hold the state after D9; recompute D7 .. D11 here step by step from the GPU's own planes instead, and
-    # compare the planes the oracle still has at the end of its frame: bokeh0/1 (after D10) and the output
-    b0, b1 = d.empty(hh, hw, 4), d.empty(hh, hw, 4)
-    capi.check(L.dfx_pass_dof_bokeh(None, cams, C.byref(a), FLAGS, 0, C.byref(d.plane(fg)), C.byref(d.plane(bg)), P(o.get("dof_in")), C.byref(d.plane(b0)),
-                                    C.byref(d.plane(b1)), rows(hh)), "D8")
-    capi.check(L.dfx_pass_dof_bokeh(None, cams, C.byref(a), FLAGS, 1, C.byref(d.plane(b0)), C.byref(d.plane(b1)), None, C.byref(d.plane(fg)),
-                                    C.byref(d.plane(bg)), rows(hh)), "D9")
-    assert_close("foreground after the flood fill", d.host(fg), o.get("dof_pre0"), tol=1e-4, max_outliers=2e-3, hdr=True)
-    assert_close("background after the flood fill", d.host(bg), o.get("dof_pre1"), tol=1e-4, max_outliers=2e-3, hdr=True)
-    capi.check(L.dfx_pass_dof_postfilter(None, C.byref(d.plane(fg)), C.byref(d.plane(bg)), C.byref(d.plane(b0)), C.byref(d.plane(b1)), rows(hh)), "D10")
-    assert_close("near layer", d.host(b0), o.get("dof_bokeh0"), tol=1e-4, max_outliers=2e-3, hdr=True)
-    assert_close("far layer", d.host(b1), o.get("dof_bokeh1"), tol=1e-4, max_outliers=2e-3, hdr=True)
-    out = d.empty(H, W, 4)
-    capi.check(L.dfx_pass_dof_combine(None, C.byref(a), P(o.get("dof_in")), C.byref(d.plane(b0)), C.byref(d.plane(b1)), C.byref(d.plane(out)), rows(H)), "D11")
-    assert_close("depth of field output", d.host(out), o.get("dof_out"), tol=1e-4, max_outliers=2e-3, min_psnr=70.0, hdr=True)
+    o, res = run_sequence(seq, v)
+    assert_default(res, v, "D")
+    L, P, g, a = capi.load(), Planes("tight"), o.get, v.dof_attribs
+    cams = P.cameras(fr["curr_camera"], fr["prev_camera"])
+    src, coc = P.up(g("dof_in")), P.up(g(f"dof_coc_temporal{fr['frame'] & 1}"))
+    l3, tmp = P.like(g("dof_dilation3")), P.like(g("dof_dilation3"))
+    fg, bg, b0, b1 = (P.like(g("dof_pre0")) for _ in range(4))
+    out = P.like(g("dof_out"))
+    r3, rh = capi.Rows(0, H >> 3), capi.Rows(0, H // 2)
+    capi.check(L.dfx_pass_dof_dilation(None, P.up(g("dof_dilation2")).ref, l3.ref, r3), "D4.3")
+    capi.check(L.dfx_pass_dof_blur_coc(None, l3.ref, 0, tmp.ref, r3), "D5")
+    capi.check(L.dfx_pass_dof_blur_coc(None, tmp.ref, 1, l3.ref, r3), "D6")
+    assert L.dfx_pass_dof_blur_coc(None, l3.ref, 1, l3.ref, r3) == capi.DFX_ERR_INVALID_ARG  # not in-place
+    capi.check(L.dfx_pass_dof_prefilter(None, src.ref, coc.ref, P.up(g("dof_dilation3")).ref, fg.ref, bg.ref, rh), "D7")
+    capi.check(L.dfx_pass_dof_bokeh(None, cams, C.byref(a), FLAGS, 0, fg.ref, bg.ref, src.ref, b0.ref, b1.ref, rh), "D8")
+    capi.check(L.dfx_pass_dof_bokeh(None, cams, C.byref(a), FLAGS, 1, b0.ref, b1.ref, None, fg.ref, bg.ref, rh), "D9")
+    chained = {"D6 chained": (l3.host(), g("dof_dilation3")), "D9 chained.near": (fg.host(), g("dof_pre0")), "D9 chained.far": (bg.host(), g("dof_pre1"))}
+    capi.check(L.dfx_pass_dof_postfilter(None, fg.ref, bg.ref, b0.ref, b1.ref, rh), "D10")
+    capi.check(L.dfx_pass_dof_combine(None, C.byref(a), src.ref, b0.ref, b1.ref, out.ref, capi.Rows(0, H)), "D11")
+    chained.update({"D10 chained.near": (b0.host(), g("dof_bokeh0")), "D10 chained.far": (b1.host(), g("dof_bokeh1")), "D11 chained": (out.host(), g("dof_out"))})
+    assert_default(chained, v, "D")
 
 
 @pytest.mark.gpu

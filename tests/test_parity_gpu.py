@@ -1,12 +1,14 @@
 """GPU parity tests: every CUDA pass against the CPU oracle on identical seeded inputs, through the C-ABI.
 
 Two layers:
-  * isolated passes — the oracle runs 4 consecutive frames; at the last frame each CUDA pass is fed the ORACLE's own
-    input planes, so a difference is attributable to that pass alone;
-  * whole chain — the effect-level objects run the same 4 frames end to end and every stage output is compared.
+  * isolated passes - at the default attribute values (and variants for the AO algorithm, the SSR ray source and the TAA flags)
+    the oracle runs the first 3 frames; gpu_frame.run_frame then steps it through the 4th pass by pass and feeds each CUDA pass
+    the ORACLE's own input planes, so a difference is attributable to that pass alone; each test checks the outputs of the passes
+    it names to the default bounds of gpu_frame.tolerance. The launch shapes and kernels selected by dfx_tune come next;
+  * whole chain - the effect-level objects run 4 frames end to end and every stage output is compared.
 
 Tolerances (fp32 arithmetic on both sides; the GPU contracts a*b+c into FMA and uses CUDA's libm, so results differ in
-the last bits; a handful of pixels may flip a discrete decision — nearest-mip rounding, a clamp, a Hi-Z cell step):
+the last bits; a handful of pixels may flip a discrete decision - nearest-mip rounding, a clamp, a Hi-Z cell step):
 per plane an absolute tolerance, a maximum fraction of outlier pixels, and a PSNR floor. HDR planes are compared after
 Reinhard c/(1+c) with peak 1 (SURVEY.md §8d). The north-star floor for the final LDR frame is 49 dB.
 """
@@ -14,9 +16,12 @@ import ctypes as C
 
 import numpy as np
 import pytest
+import torch
 
 from diligentfx_b200 import capi, synth
-from helpers import Dev, assert_close, psnr, reinhard, rows
+from gpu_frame import Planes, assert_default, run_sequence
+from helpers import assert_close, psnr
+from oracle.refshader.driver import Variant
 
 pytestmark = pytest.mark.gpu
 
@@ -41,150 +46,145 @@ def ctx(request, built):
     return dict(w=w, h=h, seq=seq, fr=seq[-1], o=o, f=seq[-1]["frame"])
 
 
-def _slots(f):
-    return f & 1, (f + 1) & 1
-
-
 # =====================================================================================================================
 # isolated passes
 # =====================================================================================================================
+# The variants beside the defaults: the other two AO algorithms, the previous-frame SSR rays and the other two TAA flag sets
+# (2 bicubic, 0 bilinear, 7 bicubic + YCoCg + Gaussian), two of them per variant.
+VARIANTS = {"default": Variant,
+            "hbao-previous_frame-bilinear": lambda: Variant(ssao_algorithm=1, ssr_flags=capi.SSR_FLAG_PREVIOUS_FRAME, taa_flags=0),
+            "vbao-ycocg-gauss": lambda: Variant(ssao_algorithm=2, taa_flags=7)}
+
+
+def _passes(ctx, variant: str = "default"):
+    """(run_frame result, variant) of the last frame of the context's sequence, the oracle having run the frames before it; once per
+    variant and size."""
+    runs = ctx.setdefault("runs", {})
+    if variant not in runs:
+        v = VARIANTS[variant]()
+        runs[variant] = (run_sequence(ctx["seq"], v)[1], v)
+    return runs[variant]
+
+
 def test_postfx_blue_noise(ctx):
-    d, o = Dev(), ctx["o"]
-    blob = np.frombuffer(open(capi.REPO_ROOT + "/diligentfx_b200/data/blue_noise_tables.bin", "rb").read(), np.uint8)
-    tables = d.torch.from_numpy(blob.copy()).cuda()
-    xy, zw = d.empty(128, 128, 2), d.empty(128, 128, 2)
-    for frame in (ctx["f"], 0, 200, 1000):
-        capi.check(d.lib.dfx_pass_blue_noise(None, C.c_void_p(tables.data_ptr()), frame, C.byref(d.plane(xy)), C.byref(d.plane(zw))))
+    """P0 at the sequence's frame and at frame indices far from it: the integer table lookups are exact; the golden-ratio shifts are
+    fp32 and may differ by an ulp, and frac() can wrap."""
+    from oracle import oracle_py as op
+    assert_default(*_passes(ctx), "P0")
+    L, P, o = capi.load(), Planes("tight"), op.Oracle(ctx["w"], ctx["h"], threads=2)
+    tables = torch.from_numpy(np.fromfile(op.TABLES, np.uint8)).cuda()
+    xy, zw = P.new(128, 128, 2), P.new(128, 128, 2)
+    for frame in (0, 200, 1000):
+        capi.check(L.dfx_pass_blue_noise(None, C.c_void_p(tables.data_ptr()), frame, xy.ref, zw.ref))
         o.set_frame_index(frame)
         o.run("blue_noise")
-        # integer table lookups are exact; the golden-ratio shifts are fp32 and may differ by an ulp, and frac() can wrap
-        for name, got in (("bn_xy", d.host(xy)), ("bn_zw", d.host(zw))):
-            want = o.get(name)
-            diff = np.abs(got - want)
+        for name, got in (("bn_xy", xy.host()), ("bn_zw", zw.host())):
+            diff = np.abs(got - o.get(name))
             diff = np.minimum(diff, 1.0 - diff)
             assert diff.max() < 1e-4, (name, frame, diff.max())
-    o.set_frame_index(ctx["f"])
-    o.run("blue_noise")
 
 
 def test_postfx_prepare(ctx):
-    d, o, fr, h, w = Dev(), ctx["o"], ctx["fr"], ctx["h"], ctx["w"]
-    cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
-    depth, prev_in, motion = d.up(fr["depth"]), d.up(fr["prev_depth"]), d.up(fr["motion"])
-    rp, cm, pd = d.empty(h, w), d.empty(h, w, 2), d.empty(h, w)
-    capi.check(d.lib.dfx_pass_postfx_prepare(None, cams, C.byref(d.plane(depth)), C.byref(d.plane(prev_in)), C.byref(d.plane(motion)), C.byref(d.plane(rp)),
-                                             C.byref(d.plane(cm)), C.byref(d.plane(pd)), rows(h)))
-    assert_close("reprojected_depth", d.host(rp), o.get("reproj_depth"), tol=2e-6)
-    assert np.array_equal(d.host(cm), o.get("closest_motion"))
-    assert np.array_equal(d.host(pd), o.get("prev_depth"))
-
-
-def _pyr_names(o, base, n):
-    return [o.get(f"{base}.{i}") for i in range(n)]
+    assert_default(*_passes(ctx), "P1", "P2", "P3")
 
 
 def test_ssao_prefilter(ctx):
-    d, o, fr, h = Dev(), ctx["o"], ctx["fr"], ctx["h"]
-    cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
-    want = _pyr_names(o, "ssao_pre", 5)
-    lv = [d.up(fr["depth"])] + [d.empty(m.shape[0], m.shape[1]) for m in want[1:]]
-    a = capi.SSAOAttribs.default()
-    capi.check(d.lib.dfx_pass_ssao_prefilter_depth(None, cams, C.byref(a), C.byref(d.pyr(lv)), rows(h)))
-    for i in range(1, 5):
-        # depth near 1.0: fp32 resolution 6e-8; the weighted view-space average amplifies rounding through 1/z
-        assert_close(f"prefiltered mip {i}", d.host(lv[i]), want[i], tol=2e-6, max_outliers=1e-3, min_psnr=100.0)
+    assert_default(*_passes(ctx), "A1")
 
 
 @pytest.mark.parametrize("algo", [0, 1, 2], ids=["GTAO", "HBAO", "VBAO"])
 def test_ssao_ambient_occlusion(ctx, algo):
-    d, o, fr, h, w = Dev(), ctx["o"], ctx["fr"], ctx["h"], ctx["w"]
-    cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
-    a = capi.SSAOAttribs.default()
-    a.Algorithm = algo
-    o.set_ssao(a)
-    o.run("ssao_ao")
-    want = o.get("ssao_occ")
-    lv = [d.up(m) for m in _pyr_names(o, "ssao_pre", 5)]
-    normal, bn, out = d.up(fr["normal"]), d.up(o.get("bn_zw")), d.empty(h, w)
-    capi.check(d.lib.dfx_pass_ssao_ambient_occlusion(None, cams, C.byref(a), C.byref(d.pyr(lv)), C.byref(d.plane(normal)), C.byref(d.plane(bn)),
-                                                     C.byref(d.plane(out)), rows(h)))
-    got = d.host(out)
-    # a tap whose LOD sits on x.5 or whose UV sits on a texel edge may pick the neighbouring texel/mip: rare, bounded
-    msg = assert_close(f"AO algo {algo}", got, want, tol=2e-3, max_outliers=(5e-3 if algo != 2 else 3e-2), min_psnr=(55.0 if algo != 2 else 40.0))
-    print(msg)
-    assert np.array_equal(got == 1.0, want == 1.0) or (np.abs((got == 1.0).astype(int) - (want == 1.0).astype(int)).mean() < 1e-3)
-    o.set_ssao(capi.SSAOAttribs.default())
-    o.run("ssao_ao")
+    assert_default(*_passes(ctx, ("default", "hbao-previous_frame-bilinear", "vbao-ycocg-gauss")[algo]), "A2")
 
 
 def test_ssao_temporal(ctx):
-    d, o, fr, h, w = Dev(), ctx["o"], ctx["fr"], ctx["h"], ctx["w"]
-    cur, prv = _slots(ctx["f"])
-    cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
-    a = capi.SSAOAttribs.default()
-    ins = [d.up(o.get(n)) for n in ("ssao_occ", f"ssao_hist{prv}", f"ssao_histlen{prv}", "reproj_depth", "prev_depth")]
-    mv = d.up(o.get("closest_motion"))
-    oo, oh = d.empty(h, w), d.empty(h, w)
-    capi.check(d.lib.dfx_pass_ssao_temporal(None, cams, C.byref(a), *[C.byref(d.plane(t)) for t in ins], C.byref(d.plane(mv)), C.byref(d.plane(oo)),
-                                            C.byref(d.plane(oh)), rows(h)))
-    # the 1 % depth-similarity test and the variance-clamp comparison are discrete decisions
-    print(assert_close("ssao accumulated", d.host(oo), o.get("ssao_acc"), tol=1e-4, max_outliers=2e-3, min_psnr=60.0))
-    print(assert_close("ssao history length", d.host(oh) / 16.0, o.get(f"ssao_histlen{cur}") / 16.0, tol=1e-4, max_outliers=2e-3, min_psnr=50.0))
+    assert_default(*_passes(ctx), "A5")
 
 
 def test_ssao_convolute_resample_spatial(ctx):
-    d, o, fr, h, w = Dev(), ctx["o"], ctx["fr"], ctx["h"], ctx["w"]
-    cur, _ = _slots(ctx["f"])
-    cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
-    a = capi.SSAOAttribs.default()
-    wocc, wdep = _pyr_names(o, "ssao_conv_occ", 5), _pyr_names(o, "ssao_conv_depth", 5)
-    occ = [d.up(wocc[0])] + [d.empty(*m.shape) for m in wocc[1:]]
-    dep = [d.up(wdep[0])] + [d.empty(*m.shape) for m in wdep[1:]]
-    capi.check(d.lib.dfx_pass_ssao_convolute(None, C.byref(d.pyr(occ)), C.byref(d.pyr(dep)), rows(h)))
-    for i in range(1, 5):
-        assert_close(f"conv occ mip {i}", d.host(occ[i]), wocc[i], tol=1e-6)
-        assert_close(f"conv depth mip {i}", d.host(dep[i]), wdep[i], tol=1e-6)
-    # A7 on the oracle's pyramids
-    occ = [d.up(m) for m in wocc]
-    dep = [d.up(m) for m in wdep]
-    hist, normal = d.up(o.get(f"ssao_histlen{cur}")), d.up(fr["normal"])
-    res = d.empty(h, w)
-    capi.check(d.lib.dfx_pass_ssao_resample(None, cams, C.byref(d.pyr(occ)), C.byref(d.pyr(dep)), C.byref(d.plane(hist)), C.byref(d.plane(normal)),
-                                            C.byref(d.plane(res)), rows(h)))
-    print(assert_close("ssao resampled", d.host(res), o.get("ssao_resampled"), tol=2e-4, max_outliers=2e-3, min_psnr=60.0))
-    # A8 on the oracle's resampled plane
-    ins = [d.up(o.get("ssao_resampled")), hist, d.up(fr["depth"]), normal]
-    out = d.empty(h, w)
-    capi.check(d.lib.dfx_pass_ssao_spatial(None, cams, C.byref(a), *[C.byref(d.plane(t)) for t in ins], C.byref(d.plane(out)), rows(h)))
-    print(assert_close("ssao spatial (output)", d.host(out), o.get("ssao_out"), tol=2e-4, max_outliers=2e-3, min_psnr=60.0))
+    assert_default(*_passes(ctx), "A6", "A7", "A8")
 
 
+def test_ssr_hiz_and_mask(ctx):
+    assert_default(*_passes(ctx), "S1", "S2")
+
+
+@pytest.mark.parametrize("flags", [0, 1], ids=["current", "previous_frame"])
+def test_ssr_intersect(ctx, flags):
+    assert_default(*_passes(ctx, ("default", "hbao-previous_frame-bilinear")[flags]), "S4")
+
+
+def test_ssr_spatial_temporal_bilateral(ctx):
+    assert_default(*_passes(ctx), "S5", "S6", "S7")
+
+
+def test_bloom_passes(ctx):
+    """B1-B4, and the same levels through the two pyramid launch shapes (one thread-block cluster / one cooperative grid)."""
+    assert_default(*_passes(ctx), "B1", "B2", "B3", "B4")
+
+
+@pytest.mark.parametrize("flags", [2, 0, 7], ids=["bicubic", "bilinear", "bicubic+ycocg+gauss"])
+def test_taa(ctx, flags):
+    """T1 separate and fused with the compose."""
+    assert_default(*_passes(ctx, {2: "default", 0: "hbao-previous_frame-bilinear", 7: "vbao-ycocg-gauss"}[flags]), "T1")
+
+
+def test_compose_and_tonemap(ctx):
+    """C1 and M1 (separate and fused with the Bloom composite) on the sequence, then all 12 operators, sRGB on and off, on random HDR
+    colour spanning 2^-8 .. 2^6 and random alpha: alpha passes through, RGB within 2e-5 of the oracle (relative to the peak above 1)."""
+    from oracle import oracle_py as op
+    assert_default(*_passes(ctx), "C1", "M1")
+    L, P = capi.load(), Planes("tight")
+    rng = np.random.default_rng(1)
+    hdr = np.zeros((64, 256, 4), np.float32)
+    hdr[..., :3] = np.exp2(rng.uniform(-8, 6, (64, 256, 3)))
+    hdr[..., 3] = rng.uniform(size=(64, 256))
+    src = P.up(hdr)
+    o = op.Oracle(256, 64, threads=2)
+    o.set("tonemap_in", hdr)
+    for mode in range(12):
+        for srgb in (0, 1):
+            a = capi.ToneMapAttribs.default()
+            a.iToneMappingMode = mode
+            o.set_tonemap(a, 0.3, bool(srgb))
+            o.run("tonemap")
+            got = P.new(64, 256, 4)
+            capi.check(L.dfx_pass_tonemap(None, C.byref(a), C.c_float(0.3), srgb, src.ref, got.ref, capi.Rows(0, 64)))
+            want, g = o.get("ldr"), got.host()
+            assert np.array_equal(g[..., 3], want[..., 3])
+            scale = max(1.0, float(np.abs(want[..., :3]).max()))
+            assert np.abs(g[..., :3] - want[..., :3]).max() <= 2e-5 * scale, (mode, srgb, np.abs(g[..., :3] - want[..., :3]).max())
+
+
+# =====================================================================================================================
+# launch shapes
+# =====================================================================================================================
 def test_pyramid_launch_shapes_agree(built):
     """The three depth / AO pyramids through their three launch shapes (dfx_tune "pyramid_impl": 2 = one TMA-staged tile kernel for the
     even levels + cluster tail, 1 = the same with plain loads, 0 = one launch per level - what the chain executor uses when the SSR and
     SSAO halves of the frame share the GPU): the same reduction per texel, so Hi-Z (a min) is bit-identical and the two averaging pyramids
     agree to rounding. 512x288: levels 1-5 from the tile kernel; 320x432: level 4 onward odd-sized."""
-    d = Dev()
-    L = d.lib
+    P = Planes("tight")
+    L = capi.load()
     a = capi.SSAOAttribs.default()
     for (w, h) in ((512, 288), (320, 432)):
         fr = synth.generate_sequence(w, h, 1)[0]
-        cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
+        cams = P.cameras(fr["curr_camera"], fr["prev_camera"])
         shapes = [(max(h >> i, 1), max(w >> i, 1)) for i in range(7)]
         ao0 = np.random.default_rng(3).random((h, w), dtype=np.float32)
         got = {}
         try:
             for impl in (2, 1, 0):
                 L.dfx_tune_set(b"pyramid_impl", impl)
-                hiz = [d.up(fr["depth"])] + [d.empty(*s_, fill=-3.0) for s_ in shapes[1:]]
-                pre = [d.up(fr["depth"])] + [d.empty(*s_, fill=-3.0) for s_ in shapes[1:5]]
-                occ = [d.up(ao0)] + [d.empty(*s_, fill=-3.0) for s_ in shapes[1:5]]
-                dep = [d.up(fr["depth"])] + [d.empty(*s_, fill=-3.0) for s_ in shapes[1:5]]
-                capi.check(L.dfx_pass_ssr_hiz(None, C.byref(d.pyr(hiz)), rows(h)))
-                capi.check(L.dfx_pass_ssao_prefilter_depth(None, cams, C.byref(a), C.byref(d.pyr(pre)), rows(h)))
-                capi.check(L.dfx_pass_ssao_convolute(None, C.byref(d.pyr(occ)), C.byref(d.pyr(dep)), rows(h)))
-                d.sync()
-                got[impl] = dict(hiz=[d.host(t) for t in hiz[1:]], pre=[d.host(t) for t in pre[1:]], occ=[d.host(t) for t in occ[1:]], dep=[d.host(t) for t in dep[1:]])
+                hiz = [P.up(fr["depth"])] + [P.new(*s_, fill=-3.0) for s_ in shapes[1:]]
+                pre = [P.up(fr["depth"])] + [P.new(*s_, fill=-3.0) for s_ in shapes[1:5]]
+                occ = [P.up(ao0)] + [P.new(*s_, fill=-3.0) for s_ in shapes[1:5]]
+                dep = [P.up(fr["depth"])] + [P.new(*s_, fill=-3.0) for s_ in shapes[1:5]]
+                capi.check(L.dfx_pass_ssr_hiz(None, C.byref(P.pyramid(hiz)), capi.Rows(0, h)))
+                capi.check(L.dfx_pass_ssao_prefilter_depth(None, cams, C.byref(a), C.byref(P.pyramid(pre)), capi.Rows(0, h)))
+                capi.check(L.dfx_pass_ssao_convolute(None, C.byref(P.pyramid(occ)), C.byref(P.pyramid(dep)), capi.Rows(0, h)))
+                torch.cuda.synchronize()
+                got[impl] = dict(hiz=[t.host() for t in hiz[1:]], pre=[t.host() for t in pre[1:]], occ=[t.host() for t in occ[1:]], dep=[t.host() for t in dep[1:]])
         finally:
             L.dfx_tune_unset(b"pyramid_impl")
         for impl in (2, 1):
@@ -194,124 +194,6 @@ def test_pyramid_launch_shapes_agree(built):
                 for i, (x, y) in enumerate(zip(got[impl][name], got[0][name])):
                     err = np.abs(x - y).max()   # depth near 1.0: one ulp is 6e-8; the prefilter's view-space average amplifies it through 1/z
                     assert err <= (1e-6 if name == "pre" else 2.5e-7), f"{w}x{h} {name} level {i + 1}: impl {impl} differs from the per-level launches by {err:.2e}"
-
-
-def test_ssr_hiz_and_mask(ctx):
-    d, o, fr, h, w = Dev(), ctx["o"], ctx["fr"], ctx["h"], ctx["w"]
-    want = _pyr_names(o, "ssr_hiz", 7)
-    lv = [d.up(fr["depth"])] + [d.empty(*m.shape) for m in want[1:]]
-    capi.check(d.lib.dfx_pass_ssr_hiz(None, C.byref(d.pyr(lv)), rows(h)))
-    for i in range(1, 7):
-        assert np.array_equal(d.host(lv[i]), want[i]), f"Hi-Z mip {i} must be bit-exact (min reduction)"
-    a = capi.SSRAttribs.default()
-    rough, mask = d.empty(h, w, fill=0.0), d.empty(h, w, dtype=d.torch.uint8, fill=7)
-    capi.check(d.lib.dfx_pass_ssr_mask_roughness(None, C.byref(a), C.byref(d.plane(d.up(fr["material"]))), C.byref(d.plane(d.up(fr["depth"]))),
-                                                 C.byref(d.plane(rough)), C.byref(d.plane(mask)), rows(h)))
-    wmask = o.get("ssr_mask")
-    assert np.array_equal(d.host(mask), wmask)
-    got_r, want_r = d.host(rough), o.get("ssr_roughness")
-    assert np.array_equal(got_r[wmask > 0], want_r[wmask > 0])
-
-
-def _ssr_common(ctx, d):
-    o, fr = ctx["o"], ctx["fr"]
-    return dict(cams=d.cameras(fr["curr_camera"], fr["prev_camera"]), a=capi.SSRAttribs.default(), rough=d.up(o.get("ssr_roughness")), mask=d.mask(o.get("ssr_mask")),
-                normal=d.up(fr["normal"]), depth=d.up(fr["depth"]), wmask=o.get("ssr_mask") > 0)
-
-
-@pytest.mark.parametrize("flags", [0, 1], ids=["current", "previous_frame"])
-def test_ssr_intersect(ctx, flags):
-    d, o, fr, h, w = Dev(), ctx["o"], ctx["fr"], ctx["h"], ctx["w"]
-    c = _ssr_common(ctx, d)
-    o.set_ssr(c["a"], flags)
-    o.run("ssr_intersect")
-    hiz = [d.up(m) for m in _pyr_names(o, "ssr_hiz", 7)]
-    rad, rdir = d.empty(h, w, 4, fill=-1.0), d.empty(h, w, 4, fill=-1.0)
-    capi.check(d.lib.dfx_pass_ssr_intersect(None, c["cams"], C.byref(c["a"]), flags, C.byref(d.plane(d.up(fr["color"]))), C.byref(d.plane(c["normal"])),
-                                            C.byref(d.plane(c["rough"])), C.byref(d.plane(c["mask"])), C.byref(d.plane(d.up(o.get("bn_xy")))), C.byref(d.pyr(hiz)),
-                                            C.byref(d.plane(d.up(fr["motion"]))), C.byref(d.plane(rad)), C.byref(d.plane(rdir)), rows(h)))
-    grad, wrad, gdir, wdir = d.host(rad), o.get("ssr_radiance"), d.host(rdir), o.get("ssr_raydir")
-    m = c["wmask"]
-    assert np.all(grad[~m] == 0.0) and np.all(gdir[~m] == 0.0), "masked-out pixels keep the clear value"
-    # The Hi-Z march is a chaotic integer walk: an ulp in the ray set-up can move a hit by a cell. Compare statistically:
-    # the hit decision (confidence > 0) must agree on >= 99 % of the rays, and rays that agree must agree closely.
-    ghit, whit = grad[..., 3] > 0, wrad[..., 3] > 0
-    agree = (ghit == whit)[m].mean()
-    both = m & ghit & whit
-    dlen = np.abs(np.linalg.norm(gdir[..., :3], axis=-1) - np.linalg.norm(wdir[..., :3], axis=-1))
-    same = both & (dlen < 1e-2 * (1.0 + np.linalg.norm(wdir[..., :3], axis=-1)))
-    print(f"ssr_intersect flags={flags}: rays={m.sum()} hit agreement={agree:.4%} same-hit among both-hit={same.sum() / max(both.sum(), 1):.4%}")
-    assert agree >= 0.99
-    assert same.sum() >= 0.98 * both.sum()
-    assert_close("ssr pdf", gdir[..., 3], wdir[..., 3], tol=1e-3 * max(1.0, float(np.abs(wdir[..., 3]).max())), max_outliers=5e-3, mask=m)
-    assert_close("ssr radiance (same hit)", grad, wrad, tol=5e-3, max_outliers=5e-3, hdr=True, mask=same)
-    o.set_ssr(c["a"], 0)
-    o.run("ssr_intersect")
-
-
-def test_ssr_spatial_temporal_bilateral(ctx):
-    d, o, fr, h, w = Dev(), ctx["o"], ctx["fr"], ctx["h"], ctx["w"]
-    cur, prv = _slots(ctx["f"])
-    c = _ssr_common(ctx, d)
-    m = c["wmask"]
-    # S5
-    orad, ovar, odep = d.empty(h, w, 4, fill=0.0), d.empty(h, w, fill=0.0), d.empty(h, w, fill=0.0)
-    capi.check(d.lib.dfx_pass_ssr_spatial(None, c["cams"], C.byref(c["a"]), C.byref(d.plane(c["rough"])), C.byref(d.plane(c["mask"])), C.byref(d.plane(c["normal"])),
-                                          C.byref(d.plane(c["depth"])), C.byref(d.plane(d.up(o.get("ssr_raydir")))), C.byref(d.plane(d.up(o.get("ssr_radiance")))),
-                                          C.byref(d.plane(orad)), C.byref(d.plane(ovar)), C.byref(d.plane(odep)), rows(h)))
-    print(assert_close("ssr resolved radiance", d.host(orad), o.get("ssr_resolved_rad"), tol=2e-3, max_outliers=3e-3, min_psnr=55.0, hdr=True, mask=m))
-    print(assert_close("ssr resolved variance", d.host(ovar), o.get("ssr_resolved_var"), tol=2e-3, max_outliers=3e-3, hdr=True, mask=m))
-    print(assert_close("ssr resolved depth", d.host(odep), o.get("ssr_resolved_depth"), tol=2e-6, max_outliers=3e-3, mask=m))
-    assert np.all(d.host(orad)[~m] == 0.0), "masked-out pixels are not written"
-    # S6 (prev slots hold frame f-1 history, curr slots hold frame f-2 data that must survive where masked)
-    names = ("ssr_resolved_depth", "reproj_depth", "ssr_resolved_rad", "ssr_resolved_var", "prev_depth", f"ssr_radhist{prv}", f"ssr_varhist{prv}")
-    ins = [d.up(o.get(n)) for n in names]
-    want_rad, want_var = o.get(f"ssr_radhist{cur}"), o.get(f"ssr_varhist{cur}")
-    out_rad, out_var = d.empty(h, w, 4, fill=123.0), d.empty(h, w, fill=123.0)
-    capi.check(d.lib.dfx_pass_ssr_temporal(None, c["cams"], C.byref(c["a"]), C.byref(d.plane(c["mask"])), C.byref(d.plane(d.up(fr["motion"]))),
-                                           *[C.byref(d.plane(t)) for t in ins], C.byref(d.plane(out_rad)), C.byref(d.plane(out_var)), rows(h)))
-    assert np.all(d.host(out_rad)[~m] == 123.0) and np.all(d.host(out_var)[~m] == 123.0), "masked-out pixels are not written"
-    print(assert_close("ssr radiance history", d.host(out_rad), want_rad, tol=2e-3, max_outliers=5e-3, min_psnr=50.0, hdr=True, mask=m))
-    print(assert_close("ssr variance history", d.host(out_var), want_var, tol=2e-3, max_outliers=5e-3, hdr=True, mask=m))
-    # S7
-    out = d.empty(h, w, 4, fill=5.0)
-    capi.check(d.lib.dfx_pass_ssr_bilateral(None, c["cams"], C.byref(c["a"]), C.byref(d.plane(c["mask"])), C.byref(d.plane(c["depth"])), C.byref(d.plane(c["normal"])),
-                                            C.byref(d.plane(c["rough"])), C.byref(d.plane(d.up(want_rad))), C.byref(d.plane(d.up(want_var))), C.byref(d.plane(out)),
-                                            rows(h)))
-    got = d.host(out)
-    assert np.all(got[~m] == 0.0), "masked-out pixels hold the clear value"
-    print(assert_close("ssr output", got, o.get("ssr_out"), tol=2e-3, max_outliers=3e-3, min_psnr=55.0, hdr=True))
-
-
-def test_bloom_passes(ctx):
-    d, o = Dev(), ctx["o"]
-    a = capi.BloomAttribs.default()
-    src = o.get("bloom_in")
-    h, w = src.shape[:2]
-    mips = d.lib.dfx_bloom_mip_count(max(w // 2, 1), max(h // 2, 1), C.c_float(a.Radius))
-    want_d = [o.get(f"bloom_down{i}") for i in range(mips)]
-    want_u = [o.get(f"bloom_up{i}") for i in range(mips - 1)]
-    # B1
-    t_in, d0 = d.up(src), d.empty(*want_d[0].shape[:2], 4)
-    capi.check(d.lib.dfx_pass_bloom_prefilter(None, C.byref(a), C.byref(d.plane(t_in)), C.byref(d.plane(d0)), rows(want_d[0].shape[0])))
-    print(assert_close("bloom prefilter", d.host(d0), want_d[0], tol=1e-4, max_outliers=1e-4, min_psnr=90.0, hdr=True))
-    # B2 on the oracle's levels
-    for i in range(1, mips):
-        out = d.empty(*want_d[i].shape[:2], 4)
-        capi.check(d.lib.dfx_pass_bloom_downsample(None, C.byref(d.plane(d.up(want_d[i - 1]))), C.byref(d.plane(out)), rows(want_d[i].shape[0])))
-        assert_close(f"bloom down {i}", d.host(out), want_d[i], tol=1e-5, min_psnr=100.0, hdr=True)
-    # B3
-    top = mips - 1
-    for i in range(top, 0, -1):
-        coarser = want_u[i] if i != top else want_d[i]
-        out = d.empty(*want_u[i - 1].shape[:2], 4)
-        capi.check(d.lib.dfx_pass_bloom_upsample(None, C.byref(d.plane(d.up(want_d[i - 1]))), C.byref(d.plane(d.up(coarser))), C.byref(d.plane(out)),
-                                                 rows(want_u[i - 1].shape[0])))
-        assert_close(f"bloom up {i - 1}", d.host(out), want_u[i - 1], tol=1e-5, min_psnr=100.0, hdr=True)
-    # B4
-    out = d.empty(h, w, 4)
-    capi.check(d.lib.dfx_pass_bloom_composite(None, C.byref(a), C.byref(d.plane(t_in)), C.byref(d.plane(d.up(want_u[0]))), C.byref(d.plane(out)), rows(h)))
-    print(assert_close("bloom output", d.host(out), o.get("bloom_out"), tol=1e-5, min_psnr=100.0, hdr=True))
 
 
 def test_bloom_tail_and_streaming_kernels(built):
@@ -327,8 +209,8 @@ def test_bloom_tail_and_streaming_kernels(built):
     o.set_bloom(a)
     o.set_inputs(seq[0])
     o.frame()
-    d = Dev()
-    L = d.lib
+    P = Planes("tight")
+    L = capi.load()
     src = o.get("bloom_in")
     mips = L.dfx_bloom_mip_count(w // 2, h // 2, C.c_float(a.Radius))
     assert mips == 9
@@ -338,21 +220,20 @@ def test_bloom_tail_and_streaming_kernels(built):
     def run(impl, tail):
         L.dfx_tune_set(b"bloom_impl", impl)
         L.dfx_tune_set(b"bloom_tail", tail)
-        dn = [d.empty(*m.shape[:2], 4) for m in want_d]
-        up = [d.empty(*m.shape[:2], 4) for m in want_d]
-        pd = (capi.Plane * mips)(*[d.plane(t) for t in dn])
-        pu = (capi.Plane * mips)(*[d.plane(t) for t in up])
+        dn = [P.new(*m.shape[:2], 4) for m in want_d]
+        up = [P.new(*m.shape[:2], 4) for m in want_d]
+        pd, pu = P.array(dn), P.array(up)
         first = L.dfx_bloom_tail_first_level(pd, mips)
-        capi.check(L.dfx_pass_bloom_prefilter(None, C.byref(a), C.byref(d.plane(d.up(src))), C.byref(pd[0]), rows(dn[0].shape[0])))
+        capi.check(L.dfx_pass_bloom_prefilter(None, C.byref(a), P.up(src).ref, C.byref(pd[0]), capi.Rows(0, dn[0].p.height)))
         for i in range(1, first):
-            capi.check(L.dfx_pass_bloom_downsample(None, C.byref(pd[i - 1]), C.byref(pd[i]), rows(dn[i].shape[0])))
+            capi.check(L.dfx_pass_bloom_downsample(None, C.byref(pd[i - 1]), C.byref(pd[i]), capi.Rows(0, dn[i].p.height)))
         if first < mips:
             capi.check(L.dfx_pass_bloom_tail(None, pd, pu, first, mips))
         top = mips - 1
         for i in range(min(top, first - 1), 0, -1):
-            capi.check(L.dfx_pass_bloom_upsample(None, C.byref(pd[i - 1]), C.byref(pu[i] if i != top else pd[i]), C.byref(pu[i - 1]), rows(up[i - 1].shape[0])))
-        d.sync()
-        return first, [d.host(t) for t in dn], [d.host(t) for t in up[:-1]]
+            capi.check(L.dfx_pass_bloom_upsample(None, C.byref(pd[i - 1]), C.byref(pu[i] if i != top else pd[i]), C.byref(pu[i - 1]), capi.Rows(0, up[i - 1].p.height)))
+        torch.cuda.synchronize()
+        return first, [t.host() for t in dn], [t.host() for t in up[:-1]]
 
     try:
         first, dn, up = run(1, 1)
@@ -379,31 +260,30 @@ def test_bloom_levels_kernel(built):
     or the other depending on the surrounding code: 1 ulp differences were observed in the up-sampled levels). The kernel leaves its
     workspace zeroed (repeated launches on the same workspace give the same planes) and works on a side stream.
     1024x576 / radius 0.95: levels 1..5 exact, 6..8 generic; 1000x562: nothing exact after level 0."""
-    import torch
-    d = Dev()
-    L = d.lib
+    P = Planes("tight")
+    L = capi.load()
     a = capi.BloomAttribs.default()
     a.Radius = 0.95
     for (w, h) in ((1024, 576), (1000, 562)):
-        src = d.up(synth.generate_sequence(w, h, 1)[0]["color"])
+        src = P.up(synth.generate_sequence(w, h, 1)[0]["color"])
         mips = L.dfx_bloom_mip_count(w // 2, h // 2, C.c_float(a.Radius))
         shapes = [(max((h // 2) >> i, 1), max((w // 2) >> i, 1)) for i in range(mips)]
 
         def planes():
-            dn, up = [d.empty(*s_, 4, fill=-7.0) for s_ in shapes], [d.empty(*s_, 4, fill=-7.0) for s_ in shapes]
-            return dn, up, (capi.Plane * mips)(*[d.plane(t) for t in dn]), (capi.Plane * mips)(*[d.plane(t) for t in up])
+            dn, up = [P.new(*s_, 4, fill=-7.0) for s_ in shapes], [P.new(*s_, 4, fill=-7.0) for s_ in shapes]
+            return dn, up, P.array(dn), P.array(up)
 
         L.dfx_tune_set(b"bloom_tail", 0)
         try:
             dn, up, pd, pu = planes()
-            capi.check(L.dfx_pass_bloom_prefilter(None, C.byref(a), C.byref(d.plane(src)), C.byref(pd[0]), rows(shapes[0][0])))
+            capi.check(L.dfx_pass_bloom_prefilter(None, C.byref(a), src.ref, C.byref(pd[0]), capi.Rows(0, shapes[0][0])))
             for i in range(1, mips):
-                capi.check(L.dfx_pass_bloom_downsample(None, C.byref(pd[i - 1]), C.byref(pd[i]), rows(shapes[i][0])))
+                capi.check(L.dfx_pass_bloom_downsample(None, C.byref(pd[i - 1]), C.byref(pd[i]), capi.Rows(0, shapes[i][0])))
             top = mips - 1
             for i in range(top, 0, -1):
-                capi.check(L.dfx_pass_bloom_upsample(None, C.byref(pd[i - 1]), C.byref(pu[i] if i != top else pd[i]), C.byref(pu[i - 1]), rows(shapes[i - 1][0])))
-            d.sync()
-            want_d, want_u = [d.host(t) for t in dn], [d.host(t) for t in up[:-1]]
+                capi.check(L.dfx_pass_bloom_upsample(None, C.byref(pd[i - 1]), C.byref(pu[i] if i != top else pd[i]), C.byref(pu[i - 1]), capi.Rows(0, shapes[i - 1][0])))
+            torch.cuda.synchronize()
+            want_d, want_u = [t.host() for t in dn], [t.host() for t in up[:-1]]
         finally:
             L.dfx_tune_unset(b"bloom_tail")
 
@@ -414,14 +294,14 @@ def test_bloom_levels_kernel(built):
             sp = C.c_void_p(stream.cuda_stream) if stream is not None else None
             if stream is not None:
                 stream.wait_stream(torch.cuda.current_stream())
-            capi.check(L.dfx_pass_bloom_prefilter(sp, C.byref(a), C.byref(d.plane(src)), C.byref(pd[0]), rows(shapes[0][0])))
+            capi.check(L.dfx_pass_bloom_prefilter(sp, C.byref(a), src.ref, C.byref(pd[0]), capi.Rows(0, shapes[0][0])))
             capi.check(L.dfx_pass_bloom_levels(sp, pd, pu, 1, mips, C.c_void_p(ws.data_ptr())))
-            d.sync()
+            torch.cuda.synchronize()
             timed_out = C.c_int32(-1)
             capi.check(L.dfx_bloom_levels_check(C.c_void_p(ws.data_ptr()), C.byref(timed_out)))
             assert timed_out.value == 0
             assert ws.cpu().tolist() == [0] * 16, f"workspace not left zeroed: {ws.cpu().tolist()}"
-            got_d, got_u = [d.host(t) for t in dn], [d.host(t) for t in up[:-1]]
+            got_d, got_u = [t.host() for t in dn], [t.host() for t in up[:-1]]
             for name, got, want in [(f"down {i}", got_d[i], want_d[i]) for i in range(mips)] + [(f"up {i}", got_u[i], want_u[i]) for i in range(mips - 1)]:
                 err = np.abs(got - want) / np.maximum(np.abs(want), 1e-3)
                 assert err.max() <= 4e-7, f"{w}x{h} attempt {attempt}: level {name} differs from the per-level launch by {err.max():.2e} (relative)"
@@ -431,54 +311,9 @@ def test_bloom_levels_kernel(built):
                 assert all(np.array_equal(a_, b_) for a_, b_ in zip(got_d + got_u, first_d + first_u)), f"{w}x{h} attempt {attempt}: not reproducible"
 
 
-@pytest.mark.parametrize("flags", [2, 0, 7], ids=["bicubic", "bilinear", "bicubic+ycocg+gauss"])
-def test_taa(ctx, flags):
-    d, o, fr, h, w = Dev(), ctx["o"], ctx["fr"], ctx["h"], ctx["w"]
-    cur, prv = _slots(ctx["f"])
-    cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
-    a = capi.TAAAttribs.default()
-    o.set_taa(a, flags)
-    o.run("taa")
-    want = o.get(f"taa_accum{cur}")
-    ins = [d.up(o.get(n)) for n in ("taa_in", f"taa_accum{prv}", "closest_motion", "reproj_depth", "prev_depth")]
-    out = d.empty(h, w, 4)
-    capi.check(d.lib.dfx_pass_taa(None, cams, C.byref(a), flags, *[C.byref(d.plane(t)) for t in ins], C.byref(d.plane(out)), rows(h)))
-    got = d.host(out)
-    # the AABB ray clip and the 0.9 disocclusion threshold are discrete decisions
-    print(assert_close(f"taa rgb flags={flags}", got[..., :3], want[..., :3], tol=1e-4, max_outliers=1e-2, min_psnr=70.0, hdr=True))
-    print(assert_close(f"taa alpha flags={flags}", got[..., 3], want[..., 3], tol=1e-4, max_outliers=1e-2))
-    o.set_taa(a, 2)
-    o.run("taa")
-
-
-def test_compose_and_tonemap(ctx):
-    d, o, fr, h, w = Dev(), ctx["o"], ctx["fr"], ctx["h"], ctx["w"]
-    out = d.empty(h, w, 4)
-    capi.check(d.lib.dfx_pass_compose(None, C.byref(d.plane(d.up(fr["color"]))), C.byref(d.plane(d.up(o.get("ssr_out")))), C.byref(d.plane(d.up(o.get("ssao_out")))),
-                                      C.c_float(1.0), C.c_float(1.0), C.byref(d.plane(out)), rows(h)))
-    assert_close("composed", d.host(out), o.get("composed"), tol=1e-5, hdr=True)
-    rng = np.random.default_rng(1)
-    hdr = np.zeros((64, 256, 4), np.float32)
-    hdr[..., :3] = np.exp2(rng.uniform(-8, 6, (64, 256, 3)))
-    hdr[..., 3] = rng.uniform(size=(64, 256))
-    from oracle import oracle_py as op
-    for mode in range(12):
-        for srgb in (0, 1):
-            a = capi.ToneMapAttribs.default()
-            a.iToneMappingMode = mode
-            o2 = op.Oracle(256, 64, threads=2)
-            o2.set("tonemap_in", hdr)
-            o2.set_tonemap(a, 0.3, bool(srgb))
-            o2.run("tonemap")
-            got = d.empty(64, 256, 4)
-            capi.check(d.lib.dfx_pass_tonemap(None, C.byref(a), C.c_float(0.3), srgb, C.byref(d.plane(d.up(hdr))), C.byref(d.plane(got)), rows(64)))
-            want = o2.get("ldr")
-            g = d.host(got)
-            assert np.array_equal(g[..., 3], want[..., 3])
-            scale = max(1.0, float(np.abs(want[..., :3]).max()))
-            assert np.abs(g[..., :3] - want[..., :3]).max() <= 2e-5 * scale, (mode, srgb, np.abs(g[..., :3] - want[..., :3]).max())
-
-
+# =====================================================================================================================
+# streaming and transfer formats
+# =====================================================================================================================
 def test_streaming_pipeline_equals_frame_by_frame(ctx):
     """The double-buffered three-stream pipeline (copy-in / compute / copy-out overlapped) must return exactly what the
     one-frame-at-a-time API returns."""

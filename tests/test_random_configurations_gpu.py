@@ -1,8 +1,8 @@
 """Every CUDA pass against the oracle at the configurations the oracle is pinned at against the reference's shaders
 (driver.random_variant: random frame sizes, the edge sizes where every pyramid reaches 1 x 1, every feature flag and every
-attribute field the kernels read), on tight, padded and 128-byte-pitched planes; plus the contracts the pass-level tests of
-test_parity_gpu.py do not reach: row ranges, the fused entries against the separate passes, CUDA-graph replay against eager
-execution, and ChainConfig values reaching the kernels.
+attribute field the kernels read), on tight, padded and 128-byte-pitched planes, to the drawn bounds of gpu_frame.tolerance
+(test_parity_gpu.py runs the same driver at the default attribute values, to the default bounds); plus row ranges, the fused
+entries against the separate passes, CUDA-graph replay against eager execution, and ChainConfig values reaching the kernels.
 """
 import copy
 import ctypes as C
@@ -12,132 +12,14 @@ import pytest
 import torch
 
 from diligentfx_b200 import capi, synth
-from gpu_frame import LAYOUTS, Planes, run_frame
+from gpu_frame import LAYOUTS, Planes, failures, run_frame
 from helpers import assert_close, psnr
 from oracle.refshader.driver import EDGE_SIZES, make_oracle, random_trial, random_variant, variant_sequence
 
 pytestmark = pytest.mark.gpu
 
 TRIALS = list(range(9)) + [f"{w}x{h}" for w, h in EDGE_SIZES]
-FLOOR_PX = 4          # every outlier budget allows at least this many pixels: 0.5 % of an 8 x 8 frame is less than one pixel
-PSNR_MIN_PX = 4096    # below this many pixels one permitted outlier dominates the mean square error: the PSNR floors apply above it
-
-EXACT = dict(exact=True)
 FILMIC_ALU = 5   # DFX_TONE_MAPPING_MODE_FILMIC_ALU
-
-
-def tolerance(label: str, v) -> dict:
-    """The comparison of one pass output: the tolerance of the pass's isolated test in test_parity_gpu.py (or of the half-resolution
-    / DoF test where that pass has its own), as keyword arguments of helpers.assert_close; `masked` = compared where the SSR mask is
-    set and bit for bit elsewhere."""
-    ssr_half, vbao = bool(v.ssr_flags & capi.SSR_FLAG_HALF_RESOLUTION), v.ssao_algorithm == 2
-    table = {
-        "P0": dict(wrap=1e-4),
-        "P1": dict(tol=2e-6), "P2": EXACT, "P3": EXACT,
-        "S1": EXACT, "S2": EXACT, "S3": EXACT,
-        "S5 ssr_spatial.radiance": dict(tol=5e-3, max_outliers=5e-3, hdr=True, masked=True) if ssr_half else
-        dict(tol=2e-3, max_outliers=3e-3, min_psnr=55.0, hdr=True, masked=True),
-        "S5 ssr_spatial.variance": dict(tol=2e-3, max_outliers=3e-3, hdr=True, masked=True),
-        "S5 ssr_spatial.depth": dict(tol=2e-6, max_outliers=3e-3, masked=True),
-        "S6 ssr_temporal.radiance": dict(tol=2e-3, max_outliers=5e-3, min_psnr=50.0, hdr=True, masked=True),
-        "S6 ssr_temporal.variance": dict(tol=2e-3, max_outliers=5e-3, hdr=True, masked=True),
-        "S7": dict(tol=2e-3, max_outliers=3e-3, min_psnr=55.0, hdr=True),
-        "A0": EXACT,
-        "A1": dict(tol=2e-6, max_outliers=1e-3, min_psnr=100.0),
-        # GTAO / HBAO: 3 % outliers where test_ssao_ambient_occlusion allows 0.5 % (the PSNR floor stays). A tap's mip is
-        # log2(radius in texels) - DepthMIPSamplingOffset, rounded: the drawn offsets (down to 1) and radii (up to 3 x 2.5) send most
-        # taps to the coarse mips, where a tap on a texel edge that rounds the other way moves by a whole coarse texel. Observed on an
-        # H100: 1.9 % at HBAO, offset 1.16, radius 1.84 x 2.32, 153 x 30; the default settings stay within 0.5 %.
-        "A2": dict(tol=2e-3, max_outliers=3e-2, min_psnr=40.0) if vbao else dict(tol=2e-3, max_outliers=3e-2, min_psnr=55.0),
-        "A4": dict(tol=1e-4, max_outliers=1e-3, min_psnr=60.0),
-        "A5 ssao_temporal.occlusion": dict(tol=1e-4, max_outliers=2e-3, min_psnr=60.0),
-        # (history / 16) to 1e-4 as test_ssao_temporal compares it, 1 % outliers where it allows 0.2 %: the history length is reset or
-        # kept by the 1 % depth-similarity test, a discrete decision per pixel; on the small random frames (4 500 pixels) the few pixels
-        # whose decision flips weigh more (observed on an H100: 0.98 % at 153 x 30).
-        "A5 ssao_temporal.history": dict(tol=1e-4 * 16, max_outliers=1e-2),
-        "A6": dict(tol=1e-6),
-        "A7": dict(tol=2e-4, max_outliers=2e-3, min_psnr=60.0),
-        "A8": dict(tol=2e-4, max_outliers=2e-3, min_psnr=60.0),
-        "C1": dict(tol=1e-5, hdr=True),
-        "T1": dict(tol=1e-4, max_outliers=1e-2, min_psnr=70.0, hdr=True),
-        "D1": dict(tol=2e-5), "D2": dict(tol=2e-5, max_outliers=1e-3), "D3": EXACT, "D4": EXACT, "D5": dict(tol=1e-6), "D6": dict(tol=1e-6),
-        "D7": dict(tol=1e-4, max_outliers=2e-3, hdr=True), "D8": dict(tol=1e-4, max_outliers=2e-3, hdr=True),
-        "D9": dict(tol=1e-4, max_outliers=2e-3, hdr=True), "D10": dict(tol=1e-4, max_outliers=2e-3, hdr=True),
-        "D11": dict(tol=1e-4, max_outliers=2e-3, min_psnr=70.0, hdr=True),
-        "B1": dict(tol=1e-4, max_outliers=1e-4, min_psnr=90.0, hdr=True),
-        "B2": dict(tol=1e-5, min_psnr=95.0, hdr=True), "B3": dict(tol=1e-5, min_psnr=95.0, hdr=True),
-        "B4": dict(tol=1e-5, min_psnr=100.0, hdr=True),
-        "M1": dict(tonemap=2e-5),
-    }
-    key = max((k for k in table if label.startswith(k)), key=len)
-    return table[key]
-
-
-def _check(label: str, got: np.ndarray, want: np.ndarray, v, ssr_mask: np.ndarray) -> str | None:
-    """None when `got` passes the comparison `tolerance(label, v)` prescribes, else the reason."""
-    if got.shape != want.shape:
-        return f"{label}: shape {got.shape} vs {want.shape}"
-    fin = np.isfinite(want)
-    if not np.isfinite(got)[fin].all():
-        return f"{label}: {int((~np.isfinite(got) & fin).sum())} non-finite values where the oracle's are finite"
-    spec = dict(tolerance(label, v))
-    if spec.pop("exact", False):
-        if np.array_equal(got.view(np.uint32), want.view(np.uint32)):
-            return None
-        d = np.abs(got.astype(np.float64) - want)
-        return f"{label}: not bit-exact ({int((d > 0).sum())} values differ, max abs {np.nanmax(d):.3e})"
-    if "wrap" in spec:                                              # fractions: 0.99999 and 0.0 are neighbours
-        d = np.abs(got - want)
-        d = np.minimum(d, 1.0 - d)
-        return None if d.max() < spec["wrap"] else f"{label}: max wrapped difference {d.max():.3e}"
-    if "tonemap" in spec:
-        scale = max(1.0, float(np.abs(want[..., :3]).max()))
-        err = np.abs(got[..., :3] - want[..., :3]).max()
-        if not np.array_equal(got[..., 3], want[..., 3]) or err > spec["tonemap"] * scale:
-            return f"{label}: max abs {err:.3e} (allowed {spec['tonemap'] * scale:.3e}), alpha equal: {np.array_equal(got[..., 3], want[..., 3])}"
-        return None
-    mask = None
-    if spec.pop("masked", False):
-        mask = ssr_mask > 0
-        outside = ~mask if got.ndim == 2 else np.broadcast_to(~mask[..., None], got.shape)
-        if not np.array_equal(got[outside].view(np.uint32), want[outside].view(np.uint32)):
-            return f"{label}: texels outside the SSR mask must keep their content"
-    npx = got.shape[0] * got.shape[1]
-    spec["max_outliers"] = max(spec.get("max_outliers", 0.0), FLOOR_PX / npx)
-    if npx < PSNR_MIN_PX:
-        spec.pop("min_psnr", None)
-    try:
-        assert_close(label, got, want, mask=mask, **spec)
-    except AssertionError as e:
-        return str(e)
-    return None
-
-
-def _check_march(res: dict, trace: np.ndarray) -> list[str]:
-    """S4, as test_ssr_intersect compares it: the Hi-Z march is a chaotic integer walk, so the hit decision must agree on 99 % of the
-    traced rays and the rays that hit on both sides must hit the same point (98 %); pdf and radiance of those rays to tolerance."""
-    (grad, wrad), (gdir, wdir) = res["S4 ssr_intersect.radiance"], res["S4 ssr_intersect.raydir_pdf"]
-    m = trace > 0
-    bad = []
-    if not (np.all(grad[~m] == 0.0) and np.all(gdir[~m] == 0.0)):
-        bad.append("S4: texels outside the trace mask must hold the clear value 0")
-    ghit, whit = grad[..., 3] > 0, wrad[..., 3] > 0
-    disagree = int(((ghit != whit) & m).sum())
-    if disagree > max(0.01 * m.sum(), FLOOR_PX):
-        bad.append(f"S4: hit decisions differ on {disagree} of {int(m.sum())} rays")
-    both = m & ghit & whit
-    norm = lambda a: np.linalg.norm(a[..., :3], axis=-1)  # noqa: E731
-    same = both & (np.abs(norm(gdir) - norm(wdir)) < 1e-2 * (1.0 + norm(wdir)))
-    if (both & ~same).sum() > max(0.02 * both.sum(), FLOOR_PX):
-        bad.append(f"S4: {int((both & ~same).sum())} of {int(both.sum())} rays that hit on both sides hit different points")
-    floor = FLOOR_PX / m.size
-    for name, g_, w_, kw in (("S4 pdf", gdir[..., 3], wdir[..., 3], dict(tol=1e-3 * max(1.0, float(np.abs(wdir[..., 3]).max())), mask=m)),
-                             ("S4 radiance (same hit)", grad, wrad, dict(tol=5e-3, hdr=True, mask=same))):
-        try:
-            assert_close(name, g_, w_, max_outliers=max(5e-3, floor), **kw)
-        except AssertionError as e:
-            bad.append(str(e))
-    return bad
 
 
 def _drawn(trial):
@@ -162,13 +44,7 @@ def test_random_configuration_passes(built, trial):
     finally:
         o.set_reversed_depth(False)
     print(f"{trial}: {w}x{h} {layout} {v}")
-    trace = res["S3 ssr_stencil_half"][1] if "S3 ssr_stencil_half" in res else res["S2 ssr_stencil"][1]
-    bad = _check_march(res, trace)
-    for label, (got, want) in res.items():
-        if not label.startswith("S4"):
-            msg = _check(label, got, want, v, res["S2 ssr_stencil"][1])
-            if msg:
-                bad.append(msg)
+    bad = failures(res, v, drawn=True)
     damaged = planes.padding_damage()
     if damaged:
         bad.append(f"{damaged} planes have values written into their row padding")

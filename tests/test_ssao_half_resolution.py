@@ -4,13 +4,13 @@
 
 CPU: hand-computed known answers for the oracle's A0 / A4 and the structure of a half-resolution frame. GPU: every new
 pass against the oracle through the C-ABI, then the whole chain with the flag."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
-from helpers import Dev, assert_close, psnr, rows
 from diligentfx_b200 import capi, synth
+from gpu_frame import Planes, assert_default, run_sequence
+from helpers import psnr
+from oracle.refshader.driver import Variant
 
 W, H, FRAMES = 160, 96, 3
 
@@ -62,38 +62,14 @@ def test_oracle_half_resolution_frame_structure(built):
 
 @pytest.mark.gpu
 def test_cuda_half_resolution_passes(built):
-    seq = synth.generate_sequence(W, H, 2)
-    fr = seq[-1]
-    o = _oracle()
-    o.set_ssao_flags(capi.SSAO_FLAG_HALF_RESOLUTION)
-    for f in seq:
-        o.set_inputs(f)
-        o.frame()
-    d = Dev()
-    cams = d.cameras(fr["curr_camera"], fr["prev_camera"])
-    depth = d.up(fr["depth"])
-    hw, hh = W // 2, H // 2
-    # A0: selection of min / max, bit-exact
-    chk = d.empty(hh, hw)
-    capi.check(d.lib.dfx_pass_ssao_downsample_depth(None, C.byref(d.plane(depth)), C.byref(d.plane(chk)), rows(hh)), "A0")
-    d.sync()
-    assert np.array_equal(d.host(chk), o.get("ssao_checker"))
-    # A3 at half resolution on the oracle's pyramid
-    a = capi.SSAOAttribs.default()
-    levels = [d.up(o.get(f"ssao_pre.{i}")) for i in range(5)]
-    occ = d.empty(hh, hw, fill=-1.0)
-    capi.check(d.lib.dfx_pass_ssao_ambient_occlusion(None, cams, C.byref(a), C.byref(d.pyr(levels)), C.byref(d.plane(d.up(fr["normal"]))),
-                                                     C.byref(d.plane(d.up(o.get("bn_zw")))), C.byref(d.plane(occ)), rows(hh)), "A3")
-    d.sync()
-    assert_close("half-res AO", d.host(occ), o.get("ssao_occ"), tol=2e-3, max_outliers=2e-3, min_psnr=50.0)
-    # A4 on the oracle's half-res occlusion
-    up = d.empty(H, W, fill=-1.0)
-    capi.check(d.lib.dfx_pass_ssao_upsample(None, cams, C.byref(d.plane(depth)), C.byref(d.plane(d.up(o.get("ssao_occ")))), C.byref(d.plane(up)), rows(H)), "A4")
-    d.sync()
-    assert_close("upsampled AO", d.host(up), o.get("ssao_occ_up"), tol=1e-4, max_outliers=1e-3, min_psnr=60.0)
-    # size checks fail loudly instead of reading out of bounds
-    bad = d.empty(hh + 1, hw)
-    assert d.lib.dfx_pass_ssao_downsample_depth(None, C.byref(d.plane(depth)), C.byref(d.plane(bad)), rows(hh)) == capi.DFX_ERR_INVALID_ARG
+    """A0 (bit-exact), A2 at half resolution and A4 against the oracle on its own inputs, to the default bounds of
+    gpu_frame.tolerance; an A0 output that is not half the depth plane is refused instead of written out of bounds."""
+    v = Variant(ssao_flags=capi.SSAO_FLAG_HALF_RESOLUTION)
+    _, res = run_sequence(synth.generate_sequence(W, H, 2), v)
+    assert_default(res, v, "A0", "A2", "A4")
+    P = Planes("tight")
+    assert capi.load().dfx_pass_ssao_downsample_depth(None, P.new(H, W, fill=0.5).ref, P.new(H // 2 + 1, W // 2).ref, capi.Rows(0, H // 2)) == \
+        capi.DFX_ERR_INVALID_ARG
 
 
 @pytest.mark.gpu
