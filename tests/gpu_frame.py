@@ -9,8 +9,14 @@ Every device plane is allocated in one of three layouts:
   "padded"  one or more texels of padding per row, pitch not a multiple of 16 bytes where the texel size allows it (the TMA paths
             need a 16-byte multiple and fall back to plain loads);
   "aligned" pitch rounded up to 128 bytes, like dfx_plane_alloc (the TMA paths run).
-The padding is filled with NaN (0xA5 for the 8-bit masks): a kernel that indexes rows with the width where it should use the
-pitch, or that reads past the end of a row, turns up as a NaN or a wrong value; `Planes.padding_damage()` reports writes into it.
+The padding is filled with NaN (half NaN for the 16-bit planes, 0xA5 for the 8-bit ones): a kernel that indexes rows with the
+width where it should use the pitch, or that reads past the end of a row, turns up as a NaN or a wrong value;
+`Planes.padding_damage()` reports writes into it.
+
+`run_frame(..., native=...)` also runs every pass that reads the G-buffer a second time on the same values in the renderer's
+formats (colour and normal RGBA16F, motion RG16F, material RG8U or RGBA16F), in the same layout, and records that output as
+"<label> [native]". Every half and UNORM8 value is an fp32 value, so `twin_failures()` requires the two outputs to be identical
+bit for bit (DESIGN §3).
 
 Test infrastructure only; it never runs the reference's shaders.
 """
@@ -28,6 +34,9 @@ from oracle.refshader.driver import Variant, _count, _levels, make_oracle
 
 LAYOUTS = ("tight", "padded", "aligned")
 MASK_FILL = 0xA5
+NATIVE = " [native]"
+NATIVE_MATERIALS = ("rg8", "rgba16")     # run_frame(native=...): the material plane's format beside RGBA16F colour / normal, RG16F motion
+_NP = {torch.float32: np.float32, torch.float16: np.float16, torch.uint8: np.uint8}
 
 
 class Buf:
@@ -48,7 +57,8 @@ class Planes:
     """Allocates device planes in one layout and keeps them (and their descriptors) alive."""
 
     _FMT = {(torch.float32, 1): (capi.FORMAT_R32F, 4), (torch.float32, 2): (capi.FORMAT_RG32F, 8), (torch.float32, 4): (capi.FORMAT_RGBA32F, 16),
-            (torch.uint8, 1): (capi.FORMAT_R8U, 1)}
+            (torch.uint8, 1): (capi.FORMAT_R8U, 1), (torch.float16, 4): (capi.FORMAT_RGBA16F, 8), (torch.float16, 2): (capi.FORMAT_RG16F, 4),
+            (torch.uint8, 2): (capi.FORMAT_RG8U, 2)}
 
     def __init__(self, layout: str = "tight"):
         assert layout in LAYOUTS, layout
@@ -67,13 +77,13 @@ class Planes:
     def new(self, h: int, w: int, ch: int = 1, fill: float | np.ndarray | None = None, flags: int = 0, dtype=torch.float32) -> Buf:
         fmt, bpt = self._FMT[(dtype, ch)]
         pitch = self.pitch(w, bpt)
-        esz = 1 if dtype == torch.uint8 else 4
+        esz = torch.tensor([], dtype=dtype).element_size()
         pad_value = MASK_FILL if dtype == torch.uint8 else float("nan")
         storage = torch.full((h * pitch // esz,), pad_value, dtype=dtype, device="cuda")
         row = pitch // esz
         t = storage.as_strided((h, w) if ch == 1 else (h, w, ch), (row, 1) if ch == 1 else (row, ch, 1))
         if isinstance(fill, np.ndarray):
-            t.copy_(torch.from_numpy(np.ascontiguousarray(fill, np.uint8 if dtype == torch.uint8 else np.float32)).cuda())
+            t.copy_(torch.from_numpy(np.ascontiguousarray(fill, _NP[dtype])).cuda())
         elif fill is not None:
             t.fill_(fill)
         b = Buf(storage, t, capi.Plane(storage.data_ptr(), pitch, w, h, fmt, flags), row)
@@ -83,6 +93,11 @@ class Planes:
     def up(self, a: np.ndarray, flags: int = 0) -> Buf:
         a = np.asarray(a, np.float32)
         return self.new(a.shape[0], a.shape[1], 1 if a.ndim == 2 else a.shape[2], fill=a, flags=flags)
+
+    def native(self, a: np.ndarray) -> Buf:
+        """A plane in the format of `a`'s own type: (H, W, 4) / (H, W, 2) float16 -> RGBA16F / RG16F, (H, W, 2) uint8 -> RG8U."""
+        dtype = {np.dtype(np.float16): torch.float16, np.dtype(np.uint8): torch.uint8}[a.dtype]
+        return self.new(a.shape[0], a.shape[1], a.shape[2], fill=a, dtype=dtype)
 
     def mask(self, a: np.ndarray) -> Buf:
         return self.new(a.shape[0], a.shape[1], fill=(np.asarray(a) != 0).astype(np.uint8), dtype=torch.uint8)
@@ -124,8 +139,86 @@ def rows(h: int) -> capi.Rows:
     return capi.Rows(0, h)
 
 
+def _exactly(a: np.ndarray, narrow: np.ndarray, what: str) -> np.ndarray:
+    """`narrow` if it widens to `a` bit for bit, else a ValueError: a twin of a value the format cannot hold would not be a twin."""
+    wide = narrow.astype(np.float32) / np.float32(255.0) if narrow.dtype == np.uint8 else narrow.astype(np.float32)
+    if not np.array_equal(wide.view(np.uint32), np.ascontiguousarray(a[..., :narrow.shape[-1]], np.float32).view(np.uint32)):
+        raise ValueError(f"the {what} plane is not exactly representable in its native format: quantise the frames first")
+    return narrow
+
+
+def native_gbuffer(P: Planes, g, material: str) -> dict[str, Buf]:
+    """The G-buffer planes the oracle holds (`g` = o.get), in the renderer's formats: colour and normal RGBA16F, motion RG16F,
+    material RG8U (`material` "rg8": z = w = 0 required) or RGBA16F ("rgba16")."""
+    assert material in NATIVE_MATERIALS, material
+    out = {n: P.native(_exactly(g(n), g(n).astype(np.float16), n)) for n in ("color", "normal", "motion")}
+    m = g("material")
+    if material == "rg8":
+        if np.any(m[..., 2:].view(np.uint32)):
+            raise ValueError("an RG8U material leaves z and w at 0")
+        out["material"] = P.native(_exactly(m, np.rint(np.clip(m[..., :2], 0.0, 1.0) * 255.0).astype(np.uint8), "material"))
+    else:
+        out["material"] = P.native(_exactly(m, m.astype(np.float16), "material"))
+    return out
+
+
+def twin_failures(res: dict) -> list[str]:
+    """Every "<label> [native]" output of run_frame(..., native=...) that is not bit-identical to the output of <label>, one message each."""
+    bad = []
+    for label, (got, _) in res.items():
+        if not label.endswith(NATIVE):
+            continue
+        want = res[label[:-len(NATIVE)]][0]
+        if got.shape != want.shape:
+            bad.append(f"{label}: shape {got.shape} vs {want.shape}")
+            continue
+        diff = got.view(np.uint32) != want.view(np.uint32)
+        if diff.any():
+            i = tuple(int(k) for k in np.argwhere(diff)[0])
+            bad.append(f"{label}: {int(diff.sum())} values differ from the fp32 planes' output, first at {i}: {got[i]!r} vs {want[i]!r}")
+    return bad
+
+
+SENTINEL = 1234.5     # row-range outputs are pre-filled with it (77 for the 8-bit ones)
+
+
+def row_range_failures(P: Planes, cases: list, rng: np.random.Generator) -> list[str]:
+    """`cases`: (name, [(h, w, ch, dtype) of the outputs], launch(rows, output refs) -> status) for passes that write one output
+    texel per invocation. Each pass is called on the whole frame, on rows [y0, y1) with a random odd y0 (the 2 x 2 quad kernels see
+    a range that starts mid-quad) and on the empty range [y0, y0): the partial call must compute exactly those rows of the whole
+    call and leave every other row at the sentinel, the empty one must be a no-op returning DFX_OK. The fused Bloom composite +
+    tone map must refuse the odd y0 and then runs from y0 - 1. One message per failure."""
+    bad = []
+    for name, specs, launch in cases:
+        def run(r):
+            outs = [P.new(h, w, ch, fill=(77 if dt == torch.uint8 else SENTINEL), dtype=dt) for h, w, ch, dt in specs]
+            st = launch(r, [b.ref for b in outs])
+            torch.cuda.synchronize()
+            return st, [b.host() for b in outs]
+        st, whole = run(capi.Rows(0, specs[0][0]))
+        capi.check(st, name)
+        hh = specs[0][0]
+        y0 = int(rng.integers(1, hh // 2)) | 1
+        y1 = int(rng.integers(y0 + 1, hh))
+        if name == "bloom_composite_tonemap":
+            assert launch(capi.Rows(y0, y1), [P.new(*specs[0][:3]).ref]) == capi.DFX_ERR_UNSUPPORTED, "odd y0 must be refused"
+            y0 -= 1
+        st, part = run(capi.Rows(y0, y1))
+        capi.check(st, f"{name} rows [{y0}, {y1})")
+        for k, (a, b) in enumerate(zip(part, whole)):
+            sentinel = 77 if specs[k][3] == torch.uint8 else SENTINEL
+            if not np.array_equal(a[y0:y1].view(np.uint32), b[y0:y1].view(np.uint32)):
+                bad.append(f"{name} output {k}: rows [{y0}, {y1}) differ from the full-frame call")
+            if not (np.all(a[:y0] == sentinel) and np.all(a[y1:] == sentinel)):
+                bad.append(f"{name} output {k}: rows outside [{y0}, {y1}) were written")
+        st, empty = run(capi.Rows(y0, y0))
+        if st != capi.DFX_OK or not all(np.all(e == (77 if s[3] == torch.uint8 else SENTINEL)) for e, s in zip(empty, specs)):
+            bad.append(f"{name}: the empty range [{y0}, {y0}) must be a no-op returning DFX_OK (status {st})")
+    return bad
+
+
 def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes: Planes | None = None,
-              stages: int | None = None) -> dict[str, tuple[np.ndarray, np.ndarray]]:
+              stages: int | None = None, native: str | None = None) -> dict[str, tuple[np.ndarray, np.ndarray]]:
     """`o` holds the history of the frames before `fr` (run with o.frame()); `fr` must be the next frame of the sequence. Outputs
     that a pass leaves untouched where its mask is off (S2 roughness, S5, S6) are pre-filled with the oracle's contents from
     before the pass, so they compare bit for bit there. `planes` (optional) receives the allocations for a padding check.
@@ -133,7 +226,13 @@ def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes:
     `stages` (oracle stage bits) limits the call to the separate passes of those stages, which is what the full-size tests can
     afford: the sections of the other stages are left out on both sides, so the oracle must already hold this frame's planes the
     selected sections read (run those stages with o.frame() first). The fused entries and the Bloom launch shapes run only when
-    `stages` is None (the whole frame of `v`)."""
+    `stages` is None (the whole frame of `v`).
+
+    `native` ("rg8" / "rgba16", see native_gbuffer): every launch that reads colour, normal, motion or material runs again on the
+    native planes, the other inputs unchanged, and its output is recorded as "<label> [native]" (P1-P3, S2, S4-S7, A2, A7, A8,
+    C1, the fused compose + TAA), plus TAA on the colour itself: "T1 taa (colour)" (fp32, against the oracle's TAA on that
+    colour) and its twin, the RGBA16F TAA a chain runs without COMPOSE in its stage mask. The frame must hold values the native
+    formats hold exactly."""
     L = capi.load()
     P = planes if planes is not None else Planes(layout)
     res: dict[str, tuple[np.ndarray, np.ndarray]] = {}
@@ -152,6 +251,12 @@ def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes:
     # ---------------- PostFXContext ----------------
     depth_np = g("depth")
     depth, motion, normal, color, material = P.up(depth_np, rev), P.up(g("motion")), P.up(g("normal")), P.up(g("color")), P.up(g("material"))
+    nat = native_gbuffer(P, g, native) if native is not None else None
+
+    def twins(name: str, wide: Buf) -> list[tuple[str, Buf]]:
+        """(label suffix, plane): the fp32 G-buffer plane `name`, and with `native` its native twin."""
+        return [("", wide)] + ([(NATIVE, nat[name])] if nat else [])
+
     if stages & op.STAGE_POSTFX:
         tables = torch.from_numpy(np.fromfile(op.TABLES, np.uint8)).cuda()
         P.keep.append(tables)
@@ -159,11 +264,13 @@ def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes:
         ok(L.dfx_pass_blue_noise(None, C.c_void_p(tables.data_ptr()), fr["frame"], xy.ref, zw.ref), "blue noise")
         o.run("blue_noise")
         res["P0 blue_noise.xy"], res["P0 blue_noise.zw"] = (xy.host(), g("bn_xy")), (zw.host(), g("bn_zw"))
-        rp, cm, pd = P.new(H, W, flags=rev), P.new(H, W, 2), P.new(H, W, flags=rev)
-        ok(L.dfx_pass_postfx_prepare(None, cams, depth.ref, P.up(g("prev_depth_in"), rev).ref, motion.ref, rp.ref, cm.ref, pd.ref, rows(H)), "postfx prepare")
+        prev_in = P.up(g("prev_depth_in"), rev)
         o.run("reprojected_depth"), o.run("closest_motion"), o.run("previous_depth")
-        res["P1 reprojected_depth"], res["P2 closest_motion"], res["P3 previous_depth"] = \
-            (rp.host(), g("reproj_depth")), (cm.host(), g("closest_motion")), (pd.host(), g("prev_depth"))
+        for sfx, mv in twins("motion", motion):
+            rp, cm, pd = P.new(H, W, flags=rev), P.new(H, W, 2), P.new(H, W, flags=rev)
+            ok(L.dfx_pass_postfx_prepare(None, cams, depth.ref, prev_in.ref, mv.ref, rp.ref, cm.ref, pd.ref, rows(H)), "postfx prepare" + sfx)
+            res["P1 reprojected_depth" + sfx], res["P2 closest_motion" + sfx], res["P3 previous_depth" + sfx] = \
+                (rp.host(), g("reproj_depth")), (cm.host(), g("closest_motion")), (pd.host(), g("prev_depth"))
     reproj, closest, prev_depth = P.up(g("reproj_depth"), rev), P.up(g("closest_motion")), P.up(g("prev_depth"), rev)
 
     # ---------------- ScreenSpaceReflection ----------------
@@ -180,9 +287,10 @@ def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes:
         rough_before = g("ssr_roughness")
         o.run("ssr_mask")
         rough_np, maskf = g("ssr_roughness"), g("ssr_mask")
-        r_out, m_out = P.up(rough_before), P.new(H, W, fill=7, dtype=torch.uint8)
-        ok(L.dfx_pass_ssr_mask_roughness(None, C.byref(A), material.ref, depth.ref, r_out.ref, m_out.ref, rows(H)), "ssr mask")
-        res["S2 ssr_roughness"], res["S2 ssr_stencil"] = (r_out.host(), rough_np), (m_out.host(), maskf)
+        for sfx, mat in twins("material", material):
+            r_out, m_out = P.up(rough_before), P.new(H, W, fill=7, dtype=torch.uint8)
+            ok(L.dfx_pass_ssr_mask_roughness(None, C.byref(A), mat.ref, depth.ref, r_out.ref, m_out.ref, rows(H)), "ssr mask" + sfx)
+            res["S2 ssr_roughness" + sfx], res["S2 ssr_stencil" + sfx] = (r_out.host(), rough_np), (m_out.host(), maskf)
         rough, mask = P.up(rough_np), P.mask(maskf)
         trace_mask = mask
         if half:
@@ -194,32 +302,39 @@ def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes:
             trace_mask = P.mask(mh)
         o.run("ssr_intersect")
         rad_np, rdir_np = g("ssr_radiance"), g("ssr_raydir")
-        rad, rdir = P.like(rad_np, fill=-1.0), P.like(rdir_np, fill=-1.0)
         bn_xy = P.up(g("bn_xy"))
-        ok(L.dfx_pass_ssr_intersect(None, cams, C.byref(A), v.ssr_flags, color.ref, normal.ref, rough.ref, trace_mask.ref, bn_xy.ref, C.byref(hiz_pyr),
-                                    motion.ref, rad.ref, rdir.ref, rows(rad_np.shape[0])), "ssr intersect")
-        res["S4 ssr_intersect.radiance"], res["S4 ssr_intersect.raydir_pdf"] = (rad.host(), rad_np), (rdir.host(), rdir_np)
+        gbuf = [(motion, normal, color)] + ([(nat["motion"], nat["normal"], nat["color"])] if nat else [])
+        for sfx, (mv, nrm, col) in zip(("", NATIVE), gbuf):
+            rad, rdir = P.like(rad_np, fill=-1.0), P.like(rdir_np, fill=-1.0)
+            ok(L.dfx_pass_ssr_intersect(None, cams, C.byref(A), v.ssr_flags, col.ref, nrm.ref, rough.ref, trace_mask.ref, bn_xy.ref, C.byref(hiz_pyr),
+                                        mv.ref, rad.ref, rdir.ref, rows(rad_np.shape[0])), "ssr intersect" + sfx)
+            res["S4 ssr_intersect.radiance" + sfx], res["S4 ssr_intersect.raydir_pdf" + sfx] = (rad.host(), rad_np), (rdir.host(), rdir_np)
         pre = [g("ssr_resolved_rad"), g("ssr_resolved_var"), g("ssr_resolved_depth")]
         o.run("ssr_spatial")
         want = [g("ssr_resolved_rad"), g("ssr_resolved_var"), g("ssr_resolved_depth")]
-        outs = [P.up(p) for p in pre]
-        ok(L.dfx_pass_ssr_spatial(None, cams, C.byref(A), rough.ref, mask.ref, normal.ref, depth.ref, P.up(rdir_np).ref, P.up(rad_np).ref,
-                                  *[b.ref for b in outs], rows(H)), "ssr spatial")
-        for n_, b_, w_ in zip(("radiance", "variance", "depth"), outs, want):
-            res[f"S5 ssr_spatial.{n_}"] = (b_.host(), w_)
+        rdir_in, rad_in = P.up(rdir_np), P.up(rad_np)
+        for sfx, nrm in twins("normal", normal):
+            outs = [P.up(p) for p in pre]
+            ok(L.dfx_pass_ssr_spatial(None, cams, C.byref(A), rough.ref, mask.ref, nrm.ref, depth.ref, rdir_in.ref, rad_in.ref,
+                                      *[b.ref for b in outs], rows(H)), "ssr spatial" + sfx)
+            for n_, b_, w_ in zip(("radiance", "variance", "depth"), outs, want):
+                res[f"S5 ssr_spatial.{n_}{sfx}"] = (b_.host(), w_)
         pre = [g(f"ssr_radhist{ci}"), g(f"ssr_varhist{ci}")]
-        ins = [motion, P.up(want[2]), reproj, P.up(want[0]), P.up(want[1]), prev_depth, P.up(g(f"ssr_radhist{pi}")), P.up(g(f"ssr_varhist{pi}"))]
+        ins = [P.up(want[2]), reproj, P.up(want[0]), P.up(want[1]), prev_depth, P.up(g(f"ssr_radhist{pi}")), P.up(g(f"ssr_varhist{pi}"))]
         o.run("ssr_temporal")
         acc = [g(f"ssr_radhist{ci}"), g(f"ssr_varhist{ci}")]
-        outs = [P.up(p) for p in pre]
-        ok(L.dfx_pass_ssr_temporal(None, cams, C.byref(A), mask.ref, *[b.ref for b in ins], *[b.ref for b in outs], rows(H)), "ssr temporal")
-        res["S6 ssr_temporal.radiance"], res["S6 ssr_temporal.variance"] = (outs[0].host(), acc[0]), (outs[1].host(), acc[1])
+        for sfx, mv in twins("motion", motion):
+            outs = [P.up(p) for p in pre]
+            ok(L.dfx_pass_ssr_temporal(None, cams, C.byref(A), mask.ref, mv.ref, *[b.ref for b in ins], *[b.ref for b in outs], rows(H)), "ssr temporal" + sfx)
+            res["S6 ssr_temporal.radiance" + sfx], res["S6 ssr_temporal.variance" + sfx] = (outs[0].host(), acc[0]), (outs[1].host(), acc[1])
         o.run("ssr_bilateral")
         ssr_out_np = g("ssr_out")
-        out = P.like(ssr_out_np, fill=5.0)
-        ok(L.dfx_pass_ssr_bilateral(None, cams, C.byref(A), mask.ref, depth.ref, normal.ref, rough.ref, P.up(acc[0]).ref, P.up(acc[1]).ref, out.ref, rows(H)),
-           "ssr bilateral")
-        res["S7 ssr_bilateral"] = (out.host(), ssr_out_np)
+        acc_rad, acc_var = P.up(acc[0]), P.up(acc[1])
+        for sfx, nrm in twins("normal", normal):
+            out = P.like(ssr_out_np, fill=5.0)
+            ok(L.dfx_pass_ssr_bilateral(None, cams, C.byref(A), mask.ref, depth.ref, nrm.ref, rough.ref, acc_rad.ref, acc_var.ref, out.ref, rows(H)),
+               "ssr bilateral" + sfx)
+            res["S7 ssr_bilateral" + sfx] = (out.host(), ssr_out_np)
 
     # ---------------- ScreenSpaceAmbientOcclusion ----------------
     if stages & op.STAGE_SSAO:
@@ -242,10 +357,12 @@ def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes:
             res[f"A1 ssao_prefilter.{i}"] = (lv[i].host(), pre[i])
         o.run("ssao_ao")
         occ_np = g("ssao_occ")
-        out = P.like(occ_np, fill=-3.0)
         pyr = P.pyramid([P.up(pre[0], src_flags)] + [P.up(m) for m in pre[1:]])
-        ok(L.dfx_pass_ssao_ambient_occlusion(None, cams, C.byref(S), C.byref(pyr), normal.ref, P.up(g("bn_zw")).ref, out.ref, rows(occ_np.shape[0])), "ssao ao")
-        res["A2 ssao_ao"] = (out.host(), occ_np)
+        bn_zw = P.up(g("bn_zw"))
+        for sfx, nrm in twins("normal", normal):
+            out = P.like(occ_np, fill=-3.0)
+            ok(L.dfx_pass_ssao_ambient_occlusion(None, cams, C.byref(S), C.byref(pyr), nrm.ref, bn_zw.ref, out.ref, rows(occ_np.shape[0])), "ssao ao" + sfx)
+            res["A2 ssao_ao" + sfx] = (out.host(), occ_np)
         if ao_half:
             o.run("ssao_upsample")
             up_np = g("ssao_occ_up")
@@ -269,24 +386,28 @@ def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes:
         o.run("ssao_resample")
         rs = g("ssao_resampled")
         hl = P.up(hlen)
-        out = P.new(H, W, fill=-3.0)
         po, pdp = P.pyramid([P.up(m) for m in co]), P.pyramid([depth] + [P.up(m) for m in cd[1:]])
-        ok(L.dfx_pass_ssao_resample(None, cams, C.byref(po), C.byref(pdp), hl.ref, normal.ref, out.ref, rows(H)), "ssao resample")
-        res["A7 ssao_resample"] = (out.host(), rs)
+        for sfx, nrm in twins("normal", normal):
+            out = P.new(H, W, fill=-3.0)
+            ok(L.dfx_pass_ssao_resample(None, cams, C.byref(po), C.byref(pdp), hl.ref, nrm.ref, out.ref, rows(H)), "ssao resample" + sfx)
+            res["A7 ssao_resample" + sfx] = (out.host(), rs)
         o.run("ssao_spatial")
         ao_np = g("ssao_out")
-        out = P.new(H, W, fill=-3.0)
-        ok(L.dfx_pass_ssao_spatial(None, cams, C.byref(S), P.up(rs).ref, hl.ref, depth.ref, normal.ref, out.ref, rows(H)), "ssao spatial")
-        res["A8 ssao_spatial"] = (out.host(), ao_np)
+        rs_in = P.up(rs)
+        for sfx, nrm in twins("normal", normal):
+            out = P.new(H, W, fill=-3.0)
+            ok(L.dfx_pass_ssao_spatial(None, cams, C.byref(S), rs_in.ref, hl.ref, depth.ref, nrm.ref, out.ref, rows(H)), "ssao spatial" + sfx)
+            res["A8 ssao_spatial" + sfx] = (out.host(), ao_np)
 
     # ---------------- compose -> TAA (separate and fused) ----------------
     if stages & op.STAGE_COMPOSE:
         ssr_out, ao = P.up(g("ssr_out")), P.up(g("ssao_out"))
         scales = (C.c_float(1.0), C.c_float(1.0))                             # the oracle's compose scales (orc_create)
         o.run("compose")
-        out = P.like(g("composed"), fill=-3.0)
-        ok(L.dfx_pass_compose(None, color.ref, ssr_out.ref, ao.ref, *scales, out.ref, rows(H)), "compose")
-        res["C1 compose"] = (out.host(), g("composed"))
+        for sfx, col in twins("color", color):
+            out = P.like(g("composed"), fill=-3.0)
+            ok(L.dfx_pass_compose(None, col.ref, ssr_out.ref, ao.ref, *scales, out.ref, rows(H)), "compose" + sfx)
+            res["C1 compose" + sfx] = (out.host(), g("composed"))
     if stages & op.STAGE_TAA:
         composed = g("composed")
         o.set("taa_in", composed)
@@ -300,10 +421,21 @@ def run_frame(o: op.Oracle, fr: dict, v: Variant, layout: str = "tight", planes:
         ok(L.dfx_pass_taa(None, cams, C.byref(v.taa), v.taa_flags, P.up(composed).ref, *[b.ref for b in taa_ins], out.ref, rows(H)), "taa")
         res["T1 taa"] = (out.host(), acc_t)
         if whole:
-            out = P.like(acc_t, fill=-3.0)
-            ok(L.dfx_pass_compose_taa(None, cams, C.byref(v.taa), v.taa_flags, color.ref, ssr_out.ref, ao.ref, *scales, *[b.ref for b in taa_ins], out.ref,
-                                      rows(H)), "compose + taa")
-            res["T1 compose_taa (fused)"] = (out.host(), acc_t)
+            for sfx, col in twins("color", color):
+                out = P.like(acc_t, fill=-3.0)
+                ok(L.dfx_pass_compose_taa(None, cams, C.byref(v.taa), v.taa_flags, col.ref, ssr_out.ref, ao.ref, *scales, *[b.ref for b in taa_ins],
+                                          out.ref, rows(H)), "compose + taa" + sfx)
+                res["T1 compose_taa (fused)" + sfx] = (out.host(), acc_t)
+        if nat:
+            # TAA on the G-buffer colour itself (a chain without COMPOSE in its stage mask); the oracle's state is put back afterwards
+            o.set("taa_in", g("color"))
+            o.run("taa")
+            acc_c = g(f"taa_accum{ci}")
+            o.set("taa_in", composed), o.set(f"taa_accum{ci}", acc_t)
+            for sfx, col in twins("color", color):
+                out = P.like(acc_t, fill=-3.0)
+                ok(L.dfx_pass_taa(None, cams, C.byref(v.taa), v.taa_flags, col.ref, *[b.ref for b in taa_ins], out.ref, rows(H)), "taa (colour)" + sfx)
+                res["T1 taa (colour)" + sfx] = (out.host(), acc_c)
         post_in = acc_t
 
     # ---------------- DepthOfField ----------------

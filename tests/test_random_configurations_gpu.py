@@ -12,7 +12,7 @@ import pytest
 import torch
 
 from diligentfx_b200 import capi, synth
-from gpu_frame import LAYOUTS, Planes, failures, run_frame
+from gpu_frame import LAYOUTS, Planes, failures, row_range_failures, run_frame
 from helpers import assert_close, psnr
 from oracle.refshader.driver import EDGE_SIZES, make_oracle, random_trial, random_variant, variant_sequence
 
@@ -55,9 +55,6 @@ def test_random_configuration_passes(built, trial):
 # =====================================================================================================================
 # row ranges
 # =====================================================================================================================
-SENTINEL = 1234.5
-
-
 def _row_range_cases(P: Planes, fr: dict, o) -> list:
     """(name, [(h, w, ch, dtype) of the outputs], launch(rows, outs)) for every pass that writes one output texel per invocation."""
     L, g = capi.load(), o.get
@@ -141,33 +138,7 @@ def test_row_ranges(built):
         o.frame(op.STAGE_ALL | op.STAGE_DOF)
     L = capi.load()
     P = Planes("tight")
-    rng = np.random.default_rng(11)
-    bad = []
-    for name, specs, launch in _row_range_cases(P, fr[-1], o):
-        def run(r):
-            outs = [P.new(h, w, ch, fill=(77 if dt == torch.uint8 else SENTINEL), dtype=dt) for h, w, ch, dt in specs]
-            st = launch(r, [b.ref for b in outs])
-            torch.cuda.synchronize()
-            return st, [b.host() for b in outs]
-        st, whole = run(capi.Rows(0, specs[0][0]))
-        capi.check(st, name)
-        hh = specs[0][0]
-        y0 = int(rng.integers(1, hh // 2)) | 1                    # odd: the 2 x 2 quad kernels see a range starting mid-quad
-        y1 = int(rng.integers(y0 + 1, hh))
-        if name == "bloom_composite_tonemap":
-            assert launch(capi.Rows(y0, y1), [P.new(*specs[0][:3]).ref]) == capi.DFX_ERR_UNSUPPORTED, "odd y0 must be refused"
-            y0 -= 1
-        st, part = run(capi.Rows(y0, y1))
-        capi.check(st, f"{name} rows [{y0}, {y1})")
-        for k, (a, b) in enumerate(zip(part, whole)):
-            sentinel = 77 if specs[k][3] == torch.uint8 else SENTINEL
-            if not np.array_equal(a[y0:y1].view(np.uint32), b[y0:y1].view(np.uint32)):
-                bad.append(f"{name} output {k}: rows [{y0}, {y1}) differ from the full-frame call")
-            if not (np.all(a[:y0] == sentinel) and np.all(a[y1:] == sentinel)):
-                bad.append(f"{name} output {k}: rows outside [{y0}, {y1}) were written")
-        st, empty = run(capi.Rows(y0, y0))
-        if st != capi.DFX_OK or not all(np.all(e == (77 if s[3] == torch.uint8 else SENTINEL)) for e, s in zip(empty, specs)):
-            bad.append(f"{name}: the empty range [{y0}, {y0}) must be a no-op returning DFX_OK (status {st})")
+    bad = row_range_failures(P, _row_range_cases(P, fr[-1], o), np.random.default_rng(11))
     cams = P.cameras(fr[-1]["curr_camera"], fr[-1]["prev_camera"])
     depth = P.up(fr[-1]["depth"])
     hiz = P.pyramid([depth] + [P.new(max(H >> i, 1), max(W >> i, 1)) for i in range(1, 7)])
