@@ -244,6 +244,15 @@ class ChainStats(C.Structure):
     _fields_ = [("frames_eager", C.c_uint64), ("frames_replayed", C.c_uint64), ("graphs_built", C.c_uint64), ("graph_failures", C.c_uint64)]
 
 
+class SceneDepthRange(C.Structure):
+    """dfx_scene_depth_range == HLSL::DepthRangeI read as floats (the layout of CameraAttribs::fSceneNearZ .. fSceneFarDepth)."""
+    _fields_ = [("fSceneNearZ", C.c_float), ("fSceneFarZ", C.c_float), ("fSceneNearDepth", C.c_float), ("fSceneFarDepth", C.c_float)]
+
+    def __bool__(self) -> bool:
+        # DepthRangeCalculator::DepthRange::operator bool (DepthRangeCalculator.hpp:158-161)
+        return self.fSceneNearDepth > 0 and self.fSceneFarDepth > 0
+
+
 CHAIN_EFFECT = {"postfx": 0, "ssao": 1, "ssr": 2, "bloom": 3, "taa": 4, "dof": 5}
 assert C.sizeof(CameraAttribs) == 576 and C.sizeof(SSAOAttribs) == 48 and C.sizeof(SSRAttribs) == 48
 assert C.sizeof(BloomAttribs) == 32 and C.sizeof(TAAAttribs) == 16 and C.sizeof(ToneMapAttribs) == 48
@@ -279,6 +288,7 @@ def load(path: str = LIB_PATH) -> C.CDLL:
     lib.dfx_chain_post_stream.restype = C.c_void_p
     lib.dfx_selection_jfa_iterations.restype = C.c_uint32
     lib.dfx_selection_jfa_iterations.argtypes = [C.c_float]
+    lib.dfx_depth_range_get_buffer.restype = C.c_void_p
     for name in declared_symbols():
         if not hasattr(lib, name):
             raise DfxError(f"libdfx_b200.so does not export {name}")

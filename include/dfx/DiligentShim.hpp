@@ -150,6 +150,20 @@ private:
     const void* m_pDevice;
 };
 
+// What a shader resource binding of the reference holds for a compute pass: the views and buffers it reads. Here it only keeps
+// the pointers (DepthRangeCalculator::CreateSRB); the objects must outlive it.
+class IShaderResourceBinding
+{
+public:
+    IShaderResourceBinding(ITextureView* pDepthSRV, IBuffer* pCameraAttribs) : m_pDepthSRV{pDepthSRV}, m_pCameraAttribs{pCameraAttribs} {}
+    ITextureView* GetDepthSRV() const { return m_pDepthSRV; }
+    IBuffer*      GetCameraAttribs() const { return m_pCameraAttribs; }
+
+private:
+    ITextureView* m_pDepthSRV;
+    IBuffer*      m_pCameraAttribs;
+};
+
 // The constant blocks shared by C++ and HLSL in the reference (Shaders/**/public/*Structures.fxh, BasicStructures.fxh) with
 // their DEFAULT_VALUE()s; layouts are the byte-identical C structs of dfx_b200.h.
 namespace HLSL

@@ -653,6 +653,22 @@ DFX_API dfx_status dfx_pass_compose_final(void* stream, const dfx_camera_attribs
                                           uint32_t grid_flags, const dfx_coordinate_grid_attribs* grid_attribs, const dfx_plane* out,
                                           dfx_rows rows);
 
+/* == HLSL::DepthRangeI (Shaders/Common/public/ComputeDepthRangeStructs.fxh), read as floats: the layout of
+ * dfx_camera_attribs::fSceneNearZ .. fSceneFarDepth (16 bytes). */
+typedef struct dfx_scene_depth_range
+{
+    float fSceneNearZ, fSceneFarZ, fSceneNearDepth, fSceneFarDepth;
+} dfx_scene_depth_range;
+/* R the scene's depth range (DepthRangeCalculator::ComputeRange, DepthRangeCalculator.cpp:229-272: ClearDepthRange.csh, then
+ * ComputeDepthRange.csh). `out_dev` (device memory, 4 floats laid out as dfx_scene_depth_range) is first set to the camera's range
+ * (near Z = fFarPlaneZ, far Z = fNearPlaneZ, near depth = fFarPlaneDepth, far depth = fNearPlaneDepth), then every non-background
+ * texel (depth != fFarPlaneDepth) of `depth` (R32F) is folded in, bit for bit as the shader does: the integer min / max of asint() of
+ * the per-thread, per-row and per-16x16-group float partials of the shader's groups, and of asint(DepthToCameraZ()) of them; with
+ * reversed depth (fNearPlaneDepth > fFarPlaneDepth) the near and far depth swap. For non-negative depths that is the plain min / max;
+ * for negative depths and -0 the grouping decides. Always the whole plane: the shader's groups are anchored at row 0, so there is no
+ * row range. Passing &cameras_dev[0].fSceneNearZ writes the range into the camera, as HnComputeDepthBoundsTask does. Two launches. */
+DFX_API dfx_status dfx_pass_depth_range(void* stream, const dfx_camera_attribs* cameras_dev, const dfx_plane* depth, float* out_dev);
+
 /* Host-side pieces that the reference computes on the CPU. */
 /* HnProcessSelectionTask::Sync (HnProcessSelectionTask.cpp:71): the number of jump-flood steps for an outline width,
  * ceil(log2(max(max_distance, 1))) + 1. */
@@ -867,6 +883,23 @@ DFX_API dfx_status dfx_coordinate_grid_create(dfx_coordinate_grid** out);
 DFX_API void       dfx_coordinate_grid_destroy(dfx_coordinate_grid* fx);
 /* CoordinateGridRenderer::Render (CoordinateGridRenderer.cpp:60-103): G1 on the whole frame. */
 DFX_API dfx_status dfx_coordinate_grid_render(dfx_coordinate_grid* fx, const dfx_coordinate_grid_render_attribs* attribs);
+
+/* ---- DepthRangeCalculator (Components/interface/DepthRangeCalculator.hpp:62-176) ---- */
+typedef struct dfx_depth_range dfx_depth_range;
+/* read_back != 0 = CreateInfo::ReadBackData: every compute also copies the range to a pinned host slot (four to start with; one more
+ * whenever every slot still has a copy in flight, as the reference's read-back queue adds a staging buffer). The device buffer starts
+ * as all zeros. */
+DFX_API dfx_status dfx_depth_range_create(int32_t read_back, dfx_depth_range** out);
+DFX_API void       dfx_depth_range_destroy(dfx_depth_range* fx);
+/* ComputeRange: dfx_pass_depth_range on `depth` with cameras_dev[0] into the effect's buffer, then (with read_back) the copy to a free
+ * host slot. */
+DFX_API dfx_status dfx_depth_range_compute(dfx_depth_range* fx, void* stream, const dfx_camera_attribs* cameras_dev, const dfx_plane* depth);
+/* GetDepthRangeBuffer: the device buffer (4 floats, dfx_scene_depth_range), valid until destroy. */
+DFX_API float* dfx_depth_range_get_buffer(const dfx_depth_range* fx);
+/* GetDepthRange: the range of the latest compute whose copy has completed (all zeros before the first one; a copy that completes
+ * after a newer one does not replace it). poll != 0 first checks the
+ * copies in flight (cudaEventQuery; it never waits); poll == 0 returns what the last poll found. */
+DFX_API dfx_status dfx_depth_range_get_range(dfx_depth_range* fx, int32_t poll, dfx_scene_depth_range* out);
 
 /* ============================================================================================================ */
 /* Ingest / egress in the reference's render-target formats (Hydrogent/src/Tasks/HnBeginFrameTask.cpp:63-69: scene colour
