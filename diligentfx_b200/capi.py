@@ -149,6 +149,34 @@ ENV_MAP_TYPE_CUBE, ENV_MAP_TYPE_SPHERE = 0, 1
 ENV_MAP_OPTION_CONVERT_OUTPUT_TO_SRGB, ENV_MAP_OPTION_COMPUTE_MOTION_VECTORS, ENV_MAP_OPTION_USE_REVERSE_DEPTH = 1, 2, 4
 
 
+class BoundBoxAttribs(C.Structure):
+    """dfx_bound_box_attribs == BoundBoxAttribs (BoundBoxStructures.fxh, 96 bytes). Transform is row-major, row-vector convention."""
+    _fields_ = [("Transform", Float4x4), ("Color", C.c_float * 4), ("PatternLength", C.c_float), ("PatternMask", C.c_uint32),
+                ("Padding0", C.c_float), ("Padding1", C.c_float)]
+
+    @staticmethod
+    def make(transform=None, color=(1.0, 1.0, 1.0, 1.0), pattern_length: float = 32.0, pattern_mask: int = 0xFFFFFFFF) -> "BoundBoxAttribs":
+        """`transform`: a 4 x 4 array (None = the identity); the rest as BoundBoxRenderer::RenderAttribs (dfx_bound_box_attribs_default)."""
+        import numpy as np
+        a = BoundBoxAttribs()
+        m = np.eye(4, dtype=np.float32) if transform is None else np.asarray(transform, np.float32)
+        assert m.shape == (4, 4)
+        for r in range(4):
+            for k in range(4):
+                a.Transform.m[r][k] = float(m[r, k])
+        a.Color[:] = [float(c) for c in color]
+        a.PatternLength, a.PatternMask = float(pattern_length), int(pattern_mask) & 0xFFFFFFFF
+        return a
+
+    @staticmethod
+    def default() -> "BoundBoxAttribs":
+        return BoundBoxAttribs.make()
+
+
+# BoundBoxRenderer::OPTION_FLAGS (Components/interface/BoundBoxRenderer.hpp)
+BOUND_BOX_OPTION_CONVERT_OUTPUT_TO_SRGB, BOUND_BOX_OPTION_COMPUTE_MOTION_VECTORS, BOUND_BOX_OPTION_USE_REVERSE_DEPTH = 1, 2, 4
+
+
 # HN_VIEW_MODE (Hydrogent/interface/HnTypes.hpp): the viewer's view modes; dfx_pass_compose_view draws SCENE_DEPTH, EDGE_MAP and MESH_ID
 VIEW_MODE_SHADED, VIEW_MODE_MOTION_VECTORS, VIEW_MODE_WHITE_BASE_COLOR = 0, 14, 19
 VIEW_MODE_SCENE_DEPTH, VIEW_MODE_EDGE_MAP, VIEW_MODE_MESH_ID, VIEW_MODE_COUNT = 24, 25, 26, 27
@@ -242,7 +270,7 @@ class CoordinateGridRenderAttribs(C.Structure):
                 ("camera_dev", C.c_void_p), ("feature_flags", C.c_uint32), ("attribs", C.POINTER(CoordinateGridAttribs))]
 
 
-assert C.sizeof(DOFAttribs) == 32 and C.sizeof(CoordinateGridAttribs) == 192 and C.sizeof(SelectionAttribs) == 48 and C.sizeof(EnvMapAttribs) == 80
+assert C.sizeof(DOFAttribs) == 32 and C.sizeof(CoordinateGridAttribs) == 192 and C.sizeof(SelectionAttribs) == 48 and C.sizeof(EnvMapAttribs) == 80 and C.sizeof(BoundBoxAttribs) == 96
 
 
 class ChainConfigC(C.Structure):

@@ -253,6 +253,19 @@ class PostProcessChain:
                                                      C.byref(attribs) if attribs is not None else None), "dfx_chain_set_environment_map")
         self._env_levels = list(levels)
 
+    def set_bound_box(self, transform, color=(1.0, 1.0, 1.0, 1.0), pattern_length: float = 32.0, pattern_mask: int = 0xFFFFFFFF):
+        """Draw the selected prim's bounding box into every following frame's G-buffer before anything reads it (HnRenderBoundBoxTask):
+        B runs right after the environment map and before PostFX, in place on the frame's colour and motion planes, storing
+        (color.rgb, 0) and the box's own motion, with the reverse-depth option of cfg.postfx_flags, in every view mode. `transform`: the
+        4 x 4 row-vector matrix that takes the unit cube to the box (synth.bound_box_transform makes Hydrogent's from a prim's extent
+        and transform); `color`, `pattern_length` (pixels, finite and > 0) and `pattern_mask` are HnRenderBoundBoxTaskParams'.
+        `transform` None switches it off."""
+        if transform is None:
+            check(self.lib.dfx_chain_set_bound_box(self.chain, None), "dfx_chain_set_bound_box")
+            return
+        a = capi.BoundBoxAttribs.make(transform, color, pattern_length, pattern_mask)
+        check(self.lib.dfx_chain_set_bound_box(self.chain, C.byref(a)), "dfx_chain_set_bound_box")
+
     def run_frame(self, frame: dict) -> torch.Tensor:
         """Public one-call API: host G-buffer in, LDR device plane out (upload + execute)."""
         self.upload(frame)

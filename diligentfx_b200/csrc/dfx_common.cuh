@@ -304,6 +304,17 @@ inline bool make_view(const dfx_plane* pl, int fmt, View<T>& v)
 #define DFX_SAME_SIZE(a, b) DFX_REQUIRE((a).w == (b).w && (a).h == (b).h, "plane size mismatch: %s vs %s", #a, #b)
 
 inline bool rows_ok(dfx_rows r, int h) { return r.y0 >= 0 && r.y1 <= h && r.y0 <= r.y1; }
+// A G-buffer plane a pass writes in place in one of two formats (bytes per texel bpt32 / bpt16): its pointer, pitch and whether it is
+// the 16-bit one; false on a null, mis-pitched, misaligned or >= 2 GiB plane.
+inline bool writable(const dfx_plane* pl, int f32, int f16, int bpt32, int bpt16, char*& p, int& pitch, int& is16)
+{
+    if (!pl || !pl->ptr || pl->width <= 0 || pl->height <= 0 || (pl->format != f32 && pl->format != f16)) return false;
+    const size_t bpt = pl->format == f32 ? bpt32 : bpt16;
+    if (pl->pitch_bytes % bpt != 0 || pl->pitch_bytes < size_t(pl->width) * bpt || reinterpret_cast<uintptr_t>(pl->ptr) % bpt != 0) return false;
+    if (pl->pitch_bytes * size_t(pl->height) >= (size_t(1) << 31)) return false;
+    p = static_cast<char*>(pl->ptr), pitch = int(pl->pitch_bytes), is16 = pl->format == f16;
+    return true;
+}
 
 struct PyrView
 {
@@ -552,6 +563,22 @@ constexpr float kPi     = 3.14159265358979f;
 constexpr float kHalfPi = 1.57079632679490f;
 constexpr float kFltEps = 5.960464478e-8f;
 constexpr float kFltMax = 3.402823466e+38f;
+
+// a / b correctly rounded, without the slow-path call of div.rn.f32 (the call makes its caller spill). The quotient is formed in
+// double from a reciprocal estimate, two Newton steps and one Markstein correction, which gives the correctly rounded double
+// quotient; rounding that to float is the correctly rounded float quotient (53 >= 2 * 24 + 2 bits). Zero, infinite and NaN
+// operands go through a * (1 / b) with the exact reciprocal of 0 / inf, which gives IEEE's results for them.
+DFX_HD float div_(float a, float b)
+{
+    const double ad = a, bd = b;
+    double       y;
+    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(bd));
+    if (!(fabsf(a) <= kFltMax) || !(fabsf(b) <= kFltMax) || b == 0.0f) return float(ad * y);
+    y              = fma(y, fma(-bd, y, 1.0), y);
+    y              = fma(y, fma(-bd, y, 1.0), y);
+    const double q = ad * y;
+    return float(fma(fma(-bd, q, ad), y, q));
+}
 
 // SSAO_Common.fxh:16-23 / SSR_Common.fxh:48-55. `rev` = the depth plane carries DFX_PLANE_FLAG_REVERSED_DEPTH (the reference
 // compiles *_OPTION_INVERTED_DEPTH shader variants; here it is a uniform kernel argument: one predicated compare).

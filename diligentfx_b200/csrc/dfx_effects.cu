@@ -876,6 +876,7 @@ namespace dfx
 bool profiling_enabled();
 void set_async_compute_hint(bool on);
 dfx_status env_map_check(int32_t type, const dfx_pyramid* env_map, uint32_t options, const dfx_env_map_attribs* attribs);
+dfx_status bound_box_check(const dfx_bound_box_attribs* attribs);
 }
 
 namespace
@@ -932,6 +933,8 @@ struct dfx_chain
     dfx_pyramid           env_map{};
     uint32_t              env_options = 0;
     dfx_env_map_attribs   env{};
+    bool                  box_on = false; // dfx_chain_set_bound_box
+    dfx_bound_box_attribs box{};
     dfx_chain_stats  stats{};
 
     void drop_graphs()
@@ -1115,6 +1118,20 @@ extern "C" dfx_status dfx_chain_set_environment_map(dfx_chain* c, int32_t type, 
     c->env_on = true, c->env_type = type, c->env_map = *env_map, c->env_options = options, c->env = a;
     return DFX_OK; // graphs are keyed on (type, map, options, attribs): the next frame records or replays the matching one
 }
+extern "C" dfx_status dfx_chain_set_bound_box(dfx_chain* c, const dfx_bound_box_attribs* attribs)
+{
+    DFX_REQUIRE(c, "null argument");
+    if (!attribs)
+    {
+        c->box_on = false;
+        return DFX_OK;
+    }
+    const dfx_status st = bound_box_check(attribs);
+    if (st != DFX_OK) return st;
+    c->box_on = true, c->box = *attribs;
+    c->box.Color[3] = 0.0f; // HnRenderBoundBoxTask's PS main: float4(Color.rgb, 0.0) (HnRenderBoundBoxTask.cpp:90)
+    return DFX_OK;          // graphs are keyed on the attribs: the next frame records or replays the matching one
+}
 extern "C" dfx_status dfx_chain_get_config(const dfx_chain* c, dfx_chain_config* out)
 {
     DFX_REQUIRE(c && out, "null argument");
@@ -1166,6 +1183,7 @@ struct FrameCtx
     bool                   front;                // PostFX prepare, S1, S2 and A2 run as one pass (dfx_pass_front_prepare) before the fork
     bool                   debug;                // a renderer debug view: no SSR, SSAO, Bloom or DoF
     bool                   env;                  // E draws the environment map into the frame's colour and motion first
+    bool                   box;                  // B draws the bounding box into them next
 };
 
 // P0, then P1-P3 + S1 + S2 + A2 in one pass on `s`; SSR and SSAO Execute then skip S1 / S2 and A2
@@ -1206,6 +1224,13 @@ dfx_status record_front(const FrameCtx& x, cudaStream_t s, dfx_plane* color_out)
                               ((cfg.postfx_flags & DFX_POSTFX_FEATURE_FLAG_REVERSED_DEPTH) ? DFX_ENV_MAP_OPTION_USE_REVERSE_DEPTH : 0u);
         if ((st = dfx_pass_env_map(s, c->pfx->cams_dev, c->env_type, &c->env_map, opts, &c->env, f->depth, f->color, f->motion, dfx_rows{0, c->h})) != DFX_OK)
             return st;
+    }
+    // B (HnRenderBoundBoxTask, right after E in the same render pass): the box's colour and its own motion, in place
+    if (x.box)
+    {
+        const uint32_t opts = DFX_BOUND_BOX_OPTION_COMPUTE_MOTION_VECTORS |
+                              ((cfg.postfx_flags & DFX_POSTFX_FEATURE_FLAG_REVERSED_DEPTH) ? DFX_BOUND_BOX_OPTION_USE_REVERSE_DEPTH : 0u);
+        if ((st = dfx_pass_bound_box(s, c->pfx->cams_dev, &c->box, opts, f->depth, f->color, f->motion, dfx_rows{0, c->h})) != DFX_OK) return st;
     }
     if (x.front)
     {
@@ -1348,6 +1373,7 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
     // caller's stream, in order with what the caller does to its planes next, and the Bloom composite runs unfused before it.
     x.grid          = c->grid_flags != 0;
     x.env           = c->env_on && c->view_mode != DFX_VIEW_MODE_SCENE_DEPTH; // HnRenderEnvMapTask::IsActive (HnRenderEnvMapTask.cpp:85-94)
+    x.box           = c->box_on; // HnRenderBoundBoxTask has no IsActive: every view mode
     x.final_compose = cfg.disable_taa != 0;
     x.with_dof      = cfg.enable_dof != 0 && !x.final_compose && !debug;
     x.side_ao      = cfg.overlap && (st & DFX_CHAIN_STAGE_SSAO) && (st & DFX_CHAIN_STAGE_SSR);
@@ -1422,7 +1448,7 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
             c->post_pending[i] = false;
         }
     // ---- cameras + frame index -> device memory (kernel parameters, no copy engine; outside the recorded graphs: they change every frame)
-    if (((st & DFX_CHAIN_STAGE_POSTFX) || x.grid || x.env || compose_view_mode(c->view_mode)) && (s = launch_upload_cameras(main, f->curr_camera, f->prev_camera, f->frame_index, c->pfx->cams_dev, c->pfx->frame_dev)) != DFX_OK) return s;
+    if (((st & DFX_CHAIN_STAGE_POSTFX) || x.grid || x.env || x.box || compose_view_mode(c->view_mode)) && (s = launch_upload_cameras(main, f->curr_camera, f->prev_camera, f->frame_index, c->pfx->cams_dev, c->pfx->frame_dev)) != DFX_OK) return s;
 
     dfx_plane color{};
     bool      replayed = false;
@@ -1441,6 +1467,7 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
             append_bytes(key, &c->env_type, sizeof(c->env_type)), append_bytes(key, &c->env_map, sizeof(c->env_map));
             append_bytes(key, &c->env_options, sizeof(c->env_options)), append_bytes(key, &c->env, sizeof(c->env));
         }
+        if (x.box) key.push_back('B'), append_bytes(key, &c->box, sizeof(c->box));
         if (debug)
         {
             append_bytes(key, &c->view_mode, sizeof(c->view_mode)), append_plane(key, &c->mesh_id);

@@ -29,22 +29,6 @@ DFX_HD int kSs(int f) { return (f == 0 || f == 5) ? -1 : 1; }
 DFX_HD int kTa(int f) { return (f == 2 || f == 3) ? 2 : 1; }
 DFX_HD int kTs(int f) { return f == 2 ? 1 : -1; }
 
-// a / b correctly rounded, without the slow-path call of div.rn.f32 (the call makes its caller spill). The quotient is formed in
-// double from a reciprocal estimate, two Newton steps and one Markstein correction, which gives the correctly rounded double
-// quotient; rounding that to float is the correctly rounded float quotient (53 >= 2 * 24 + 2 bits). Zero, infinite and NaN
-// operands go through a * (1 / b) with the exact reciprocal of 0 / inf, which gives IEEE's results for them.
-DFX_HD float div_(float a, float b)
-{
-    const double ad = a, bd = b;
-    double       y;
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(bd));
-    if (!(fabsf(a) <= kFltMax) || !(fabsf(b) <= kFltMax) || b == 0.0f) return float(ad * y);
-    y              = fma(y, fma(-bd, y, 1.0), y);
-    y              = fma(y, fma(-bd, y, 1.0), y);
-    const double q = ad * y;
-    return float(fma(fma(-bd, q, ad), y, q));
-}
-
 DFX_HD float  comp(float3 v, int a) { return a == 0 ? v.x : a == 1 ? v.y : v.z; }
 DFX_HD float4 add4(float4 a, float4 b) { return make_float4(add_(a.x, b.x), add_(a.y, b.y), add_(a.z, b.z), add_(a.w, b.w)); }
 DFX_HD float4 mul4(float4 a, float w) { return make_float4(mul_(a.x, w), mul_(a.y, w), mul_(a.z, w), mul_(a.w, w)); }
@@ -229,16 +213,6 @@ __global__ void __launch_bounds__(256) env_map_kernel(const dfx_camera_attribs* 
         else
             *reinterpret_cast<float2*>(mrow) = make_float2(mx, my);
     }
-}
-
-bool writable(const dfx_plane* pl, int f32, int f16, int bpt32, int bpt16, char*& p, int& pitch, int& is16)
-{
-    if (!pl || !pl->ptr || pl->width <= 0 || pl->height <= 0 || (pl->format != f32 && pl->format != f16)) return false;
-    const size_t bpt = pl->format == f32 ? bpt32 : bpt16;
-    if (pl->pitch_bytes % bpt != 0 || pl->pitch_bytes < size_t(pl->width) * bpt || reinterpret_cast<uintptr_t>(pl->ptr) % bpt != 0) return false;
-    if (pl->pitch_bytes * size_t(pl->height) >= (size_t(1) << 31)) return false;
-    p = static_cast<char*>(pl->ptr), pitch = int(pl->pitch_bytes), is16 = pl->format == f16;
-    return true;
 }
 
 // The checks dfx_pass_env_map and dfx_chain_set_environment_map share: the type, the options, the tone-mapping mode and the map

@@ -588,3 +588,33 @@ def env_map_cameras(width: int, height: int) -> dict:
             for sz in (1, -1):
                 out[f"corner{sx:+d}{sy:+d}{sz:+d}"] = look_at_camera(eye, eye + np.array([sx, sy, sz], np.float64), width, height)
     return out
+
+
+def bound_box_transform(extent_min, extent_max, prim_transform=None) -> np.ndarray:
+    """HnRenderBoundBoxTask's box transform (HnRenderBoundBoxTask.cpp:132-139): Scale(max - min) * Translation(min) * PrimTransform, row
+    vectors, in float32 as float4x4's operator* forms it (sum over k of a[i][k] * b[k][j], k in order). `prim_transform` None = the
+    identity. The unit cube's corner c goes to float4(c, 1) * result."""
+    lo, hi = np.asarray(extent_min, np.float32), np.asarray(extent_max, np.float32)
+    scale = np.diag(np.append(hi - lo, np.float32(1.0))).astype(np.float32)
+    trans = np.eye(4, dtype=np.float32)
+    trans[3, :3] = lo
+
+    def mul(a, b):
+        out = np.zeros((4, 4), np.float32)
+        for i in range(4):
+            for j in range(4):
+                s = np.float32(a[i, 0] * b[0, j])
+                for k in range(1, 4):
+                    s = np.float32(s + np.float32(a[i, k] * b[k, j]))
+                out[i, j] = s
+        return out
+
+    m = mul(scale, trans)
+    return m if prim_transform is None else mul(m, np.asarray(prim_transform, np.float32))
+
+
+def sphere_bound_box(k: int, seed: int = 7, count: int = 24) -> np.ndarray:
+    """The box of sphere `k` of make_scene(seed, count): its extent centre -+ radius, in world space (the identity prim transform)."""
+    scene = make_scene(seed, count)
+    c, r = scene.centers[k], scene.radii[k]
+    return bound_box_transform(c - r, c + r)

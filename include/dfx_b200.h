@@ -286,6 +286,25 @@ typedef struct dfx_env_map_attribs
 #define DFX_ENV_MAP_OPTION_USE_REVERSE_DEPTH      (1u << 2)
 #define DFX_ENV_MAP_OPTION_ALL                    7u
 
+/* == BoundBoxAttribs, Shaders/Common/private/BoundBoxStructures.fxh (96 bytes): what BoundBoxRenderer::Prepare writes
+ * (Components/src/BoundBoxRenderer.cpp:224-255). Transform is the matrix as the shader reads it: a box corner c in [0, 1]^3 goes to
+ * mul(float4(c, 1), Transform) (row vector times matrix, row-major here). */
+typedef struct dfx_bound_box_attribs
+{
+    dfx_float4x4 Transform;     /* identity: the unit cube                                                    */
+    float        Color[4];      /* (1, 1, 1, 1): stored as given                                             */
+    float        PatternLength; /* 32: pixels                                                                 */
+    uint32_t     PatternMask;   /* 0xFFFFFFFF: bit k fills the k-th 1/32 of the pattern                       */
+    float        Padding0;
+    float        Padding1;
+} dfx_bound_box_attribs;
+/* BoundBoxRenderer::OPTION_FLAGS (Components/interface/BoundBoxRenderer.hpp) */
+#define DFX_BOUND_BOX_OPTION_NONE                   0u
+#define DFX_BOUND_BOX_OPTION_CONVERT_OUTPUT_TO_SRGB (1u << 0)
+#define DFX_BOUND_BOX_OPTION_COMPUTE_MOTION_VECTORS (1u << 1)
+#define DFX_BOUND_BOX_OPTION_USE_REVERSE_DEPTH      (1u << 2)
+#define DFX_BOUND_BOX_OPTION_ALL                    7u
+
 /* Default-initialisers (the reference's DEFAULT_VALUE()s). */
 DFX_API void dfx_ssao_attribs_default(dfx_ssao_attribs* a);
 DFX_API void dfx_ssr_attribs_default(dfx_ssr_attribs* a);
@@ -297,6 +316,8 @@ DFX_API void dfx_coordinate_grid_attribs_default(dfx_coordinate_grid_attribs* a)
 DFX_API void dfx_selection_attribs_default(dfx_selection_attribs* a);
 /* EnvMapRenderer::RenderAttribs' defaults (AverageLogLum 1, MipLevel 0, Alpha 1, Scale (1, 1, 1)) with dfx_tonemap_attribs_default */
 DFX_API void dfx_env_map_attribs_default(dfx_env_map_attribs* a);
+/* BoundBoxRenderer::RenderAttribs' defaults: the identity transform, Color (1, 1, 1, 1), PatternLength 32, PatternMask 0xFFFFFFFF */
+DFX_API void dfx_bound_box_attribs_default(dfx_bound_box_attribs* a);
 
 /* == PostFXContext::FrameDesc, PostProcess/Common/interface/PostFXContext.hpp:68-84 */
 typedef struct dfx_frame_desc
@@ -676,6 +697,24 @@ DFX_API dfx_status dfx_pass_copy_frame_grid(void* stream, const dfx_camera_attri
 DFX_API dfx_status dfx_pass_env_map(void* stream, const dfx_camera_attribs* cameras_dev, int32_t type, const dfx_pyramid* env_map,
                                     uint32_t options, const dfx_env_map_attribs* attribs, const dfx_plane* depth,
                                     const dfx_plane* color_inout, const dfx_plane* motion_inout, dfx_rows rows);
+
+/* B the selected prim's bounding box (Components/src/BoundBoxRenderer.cpp:150-168 GetPSO, :257-277 Render; Shaders/Common/private/
+ * BoundBox.vsh, BoundBox.psh:27-48 GetBoundBoxOutput), in place on the G-buffer's colour and motion planes. The 24 vertices of
+ * BoundBoxVS (GetBoxCorner's table through attribs->Transform, then cameras_dev[0].mViewProj; PREV_CLIP_POS through cameras_dev[1]'s)
+ * make 12 lines, rasterised by the aliased-line rule of DESIGN.md §2: clipped against 0 <= z <= w, snapped to 1/256 pixel in the
+ * plane-sized viewport, diamond exit, attributes at the pixel centre's projection onto the snapped segment. A fragment is kept when
+ * its z / w passes the depth test LESS_EQUAL (GREATER_EQUAL with DFX_BOUND_BOX_OPTION_USE_REVERSE_DEPTH; no depth write) and the
+ * pattern bit min(uint(frac(Dist / PatternLength) * PatternLength), 31) of PatternMask is set (Dist: the distance in pixels to the
+ * line's first vertex, from the interpolated clip positions); a pixel keeps the last kept fragment in primitive order. A kept
+ * pixel's colour is attribs->Color as given, and with DFX_BOUND_BOX_OPTION_COMPUTE_MOTION_VECTORS its motion is
+ * GetMotionVector(ClipPos.xy / w, PrevClipPos.xy / w, Jitter, PrevJitter); every other pixel is not touched.
+ * DFX_BOUND_BOX_OPTION_CONVERT_OUTPUT_TO_SRGB changes nothing, as in the reference (BoundBox.psh never reads it). depth R32F;
+ * color_inout RGBA32F or RGBA16F; motion_inout RG32F or RG16F (required with motion vectors; otherwise it may be NULL and is not
+ * touched); the 16-bit stores round to nearest even. Any row range; only its rows are touched, and they are the rows of a full call.
+ * Refuses unknown option bits, mismatched plane sizes, motion vectors without a motion plane, and a PatternLength that is not finite
+ * and > 0. */
+DFX_API dfx_status dfx_pass_bound_box(void* stream, const dfx_camera_attribs* cameras_dev, const dfx_bound_box_attribs* attribs, uint32_t options,
+                                      const dfx_plane* depth, const dfx_plane* color_inout, const dfx_plane* motion_inout, dfx_rows rows);
 
 /* J the closest selected location (Hydrogent/src/Tasks/HnProcessSelectionTask.cpp:304-369): HnInitClosestSelectedLocation.psh on
  * `selection_depth` (R32F; a texel != clear_depth is selected), then dfx_selection_jfa_iterations(max_distance) steps of
@@ -1144,6 +1183,13 @@ DFX_API dfx_status dfx_chain_set_view_mode(dfx_chain* chain, int32_t view_mode, 
  * dfx_pass_env_map refuses about the type, the options, the tone-mapping mode and the map. */
 DFX_API dfx_status dfx_chain_set_environment_map(dfx_chain* chain, int32_t type, const dfx_pyramid* env_map, uint32_t options,
                                                  const dfx_env_map_attribs* attribs);
+/* The selected prim's bounding box (HnRenderBoundBoxTask, Hydrogent/src/Tasks/HnRenderBoundBoxTask.cpp:107-207): attribs != NULL makes
+ * every following frame (replayed frames included) run B (dfx_pass_bound_box) right after E and before PostFX, in place on the
+ * frame's colour and motion planes, storing (Color.rgb, 0) as HnRenderBoundBoxTask's PS main does (:75-98). Motion vectors are always
+ * on; the reverse-depth option follows DFX_POSTFX_FEATURE_FLAG_REVERSED_DEPTH. B runs in every view mode (the task has no IsActive).
+ * attribs NULL switches B off (the default): the chain then issues exactly the kernels it issues without it. Refuses a PatternLength
+ * that is not finite and > 0. */
+DFX_API dfx_status dfx_chain_set_bound_box(dfx_chain* chain, const dfx_bound_box_attribs* attribs);
 
 /* ============================================================================================================ */
 /* 4. one frame split into row strips over the GPUs of a box (no reference counterpart)                          */
