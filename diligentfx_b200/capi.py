@@ -177,6 +177,29 @@ class BoundBoxAttribs(C.Structure):
 BOUND_BOX_OPTION_CONVERT_OUTPUT_TO_SRGB, BOUND_BOX_OPTION_COMPUTE_MOTION_VECTORS, BOUND_BOX_OPTION_USE_REVERSE_DEPTH = 1, 2, 4
 
 
+class VectorFieldAttribs(C.Structure):
+    """dfx_vector_field_attribs == VectorFieldRenderer::RenderAttribs' values (56 bytes): Bias, Scale, StartColor, EndColor, GridSize."""
+    _fields_ = [("Bias", C.c_float * 2), ("Scale", C.c_float * 2), ("StartColor", C.c_float * 4), ("EndColor", C.c_float * 4),
+                ("GridSize", C.c_uint32 * 2)]
+
+    @staticmethod
+    def make(grid=(0, 0), bias=(0.0, 0.0), scale=(1.0, 1.0), start_color=(1.0, 1.0, 1.0, 1.0), end_color=(1.0, 1.0, 1.0, 1.0)) -> "VectorFieldAttribs":
+        """The defaults are RenderAttribs' (dfx_vector_field_attribs_default); `grid` = (lines across, lines down)."""
+        a = VectorFieldAttribs()
+        a.Bias[:], a.Scale[:] = [float(v) for v in bias], [float(v) for v in scale]
+        a.StartColor[:], a.EndColor[:] = [float(v) for v in start_color], [float(v) for v in end_color]
+        a.GridSize[:] = [int(v) & 0xFFFFFFFF for v in grid]
+        return a
+
+    @staticmethod
+    def default() -> "VectorFieldAttribs":
+        return VectorFieldAttribs.make()
+
+
+# VectorFieldRenderer::RenderAttribs::ConvertOutputToSRGB as an option bit
+VECTOR_FIELD_OPTION_CONVERT_OUTPUT_TO_SRGB = 1
+
+
 # HN_VIEW_MODE (Hydrogent/interface/HnTypes.hpp): the viewer's view modes; dfx_pass_compose_view draws SCENE_DEPTH, EDGE_MAP and MESH_ID
 VIEW_MODE_SHADED, VIEW_MODE_MOTION_VECTORS, VIEW_MODE_WHITE_BASE_COLOR = 0, 14, 19
 VIEW_MODE_SCENE_DEPTH, VIEW_MODE_EDGE_MAP, VIEW_MODE_MESH_ID, VIEW_MODE_COUNT = 24, 25, 26, 27
@@ -271,6 +294,7 @@ class CoordinateGridRenderAttribs(C.Structure):
 
 
 assert C.sizeof(DOFAttribs) == 32 and C.sizeof(CoordinateGridAttribs) == 192 and C.sizeof(SelectionAttribs) == 48 and C.sizeof(EnvMapAttribs) == 80 and C.sizeof(BoundBoxAttribs) == 96
+assert C.sizeof(VectorFieldAttribs) == 56
 
 
 class ChainConfigC(C.Structure):

@@ -226,7 +226,8 @@ class PostProcessChain:
         this frame's depth range, which the chain computes), EDGE_MAP and MESH_ID are drawn by HnPostProcess.psh's view-mode steps;
         MESH_ID reads `mesh_id` ((H, W) float32 CUDA tensor, the renderer's mesh-ID target) every frame: write the next frame's IDs
         into it in place. `loading_animation_factor` != 0 leaves the scene-depth colour as drawn. The switch does not reset TAA.
-        MOTION_VECTORS is refused (DfxError, DFX_ERR_UNSUPPORTED)."""
+        MOTION_VECTORS is refused here (DfxError, DFX_ERR_UNSUPPORTED): it takes the frame's elapsed time, through
+        set_motion_vector_view. Any mode set here leaves the motion-vector view."""
         p = None
         if mode == capi.VIEW_MODE_MESH_ID:
             if mesh_id is None:
@@ -235,6 +236,19 @@ class PostProcessChain:
         check(self.lib.dfx_chain_set_view_mode(self.chain, int(mode), C.byref(p) if p is not None else None, C.c_float(loading_animation_factor)),
               "dfx_chain_set_view_mode")
         self._mesh_id = mesh_id if p is not None else None
+
+    def set_motion_vector_view(self, elapsed: float | None):
+        """The viewer's motion-vector view (HN_VIEW_MODE_MOTION_VECTORS) from the next frame on, with `elapsed` the frame's ElapsedTime in
+        seconds: call it again with each frame's before that frame. Whatever cfg.enable_taa says, the frame is drawn as with TAA off and no
+        PostFX, SSR or SSAO (E, B and the selection as configured): the compose with zero SSR and SSAO scales writes the LDR frame with
+        the tone map, the selection, the grid and sRGB, and then VectorFieldRenderer draws the frame's motion plane over it, one line per
+        20 x 20 pixels pointing against the motion, scaled by -0.02 / max(elapsed, 0.001), white to grey. A new elapsed time every frame
+        replays the same graph. `elapsed` None returns to SHADED; so does any set_view_mode call. The first TAA frame afterwards resets
+        TAA's history."""
+        on = elapsed is not None
+        check(self.lib.dfx_chain_set_motion_vector_view(self.chain, int(on), C.c_float(elapsed if on else 0.0)), "dfx_chain_set_motion_vector_view")
+        if on:
+            self._mesh_id = None
 
     def set_environment_map(self, env_type: int | None, levels: list | None = None, options: int = 0, attribs: capi.EnvMapAttribs | None = None):
         """Draw the environment-map background into every following frame's G-buffer before anything reads it (HnRenderEnvMapTask): E runs

@@ -8,14 +8,13 @@
 // bit for bit. Each CTA sets the 12 lines up in shared memory; then one thread per major-axis step of one line draws at most one
 // pixel. The overlap rule (a pixel keeps the last surviving fragment in primitive order) is resolved without barriers between lines:
 // a thread stores its fragment only if no later line covers its pixel with a fragment that survives the depth and pattern tests.
-#include "dfx_common.cuh"
+#include "dfx_line.cuh"
 
 namespace dfx
 {
 namespace
 {
-constexpr int   kBoxThreads = 128;
-constexpr float kGuard      = 268435456.0f; // 2^28: the guard band of 2^20 pixels in 1/256 units
+constexpr int kBoxThreads = 128;
 
 struct BoxLine
 {
@@ -53,18 +52,6 @@ DFX_HD void box_vs(uint32_t id, const dfx_camera_attribs* cams, const dfx_float4
     put4(a + 8, mul_row(box_corner(id & ~1u, T), cams[0].mViewProj));
 }
 
-// the viewport transform (y down) and the 16.8 snap (round half to even); false beyond the guard band, at w <= 0 or on NaN
-DFX_HD bool snap(const float* a, float W, float H, int& X, int& Y, float& nz, float& iw)
-{
-    if (!(a[3] > 0.0f)) return false;
-    const float nx = div_(a[0], a[3]), ny = div_(a[1], a[3]);
-    nz = div_(a[2], a[3]), iw = div_(1.0f, a[3]);
-    const float sx = mul_(mul_(add_(mul_(nx, 0.5f), 0.5f), W), 256.0f), sy = mul_(mul_(sub_(0.5f, mul_(ny, 0.5f)), H), 256.0f);
-    if (!(fabsf(sx) < kGuard) || !(fabsf(sy) < kGuard)) return false;
-    X = int(rintf(sx)), Y = int(rintf(sy));
-    return true;
-}
-
 // Line l: the VS of its two vertices, [near, far] clipping in clip space (d = z, then d = w - z; NaN is outside), the snap
 __device__ void setup_line(int l, const dfx_camera_attribs* cams, const dfx_bound_box_attribs& A, bool motion, float W, float H, BoxLine& L)
 {
@@ -95,49 +82,6 @@ __device__ void setup_line(int l, const dfx_camera_attribs* cams, const dfx_boun
     for (int k = 0; k < 12; ++k) L.a0[k] = v0[k], L.a1[k] = v1[k];
     L.xmajor = abs(L.bx - L.ax) >= abs(L.by - L.ay);
     L.ok     = 1;
-}
-
-// floor(n / d) for 0 < d < 2^30, |n| < 2^59, without a 64-bit division: a double estimate from a refined reciprocal is within 2^-15 of
-// n / d (|n / d| < 2^30), so the floor is off by at most one, which the remainder corrects
-DFX_HD long long floor_div64(long long n, long long d)
-{
-    double y;
-    const double dd = double(d);
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(dd));
-    y           = fma(y, fma(-dd, y, 1.0), y);
-    y           = fma(y, fma(-dd, y, 1.0), y);
-    long long q = (long long)floor(double(n) * y);
-    long long r = n - q * d;
-    if (r < 0) --q, r += d;
-    if (r >= d) ++q, r -= d;
-    return q;
-}
-
-// the half-open diamond of the pixel centred at (cu, cv): |du| + |dv| < 1/2, plus the right and bottom corners and the edge between them
-DFX_HD bool in_diamond(int pu, int pv, int cu, int cv)
-{
-    const long long du = (long long)pu - cu, dv = (long long)pv - cv, s = llabs(du) + llabs(dv);
-    return s < 128 || (s == 128 && du >= 0 && dv >= 0);
-}
-
-// major-axis step i, in the frame where the major axis is u: the minor pixel j the line draws there, or false (DESIGN.md §2)
-DFX_HD bool step_pixel(int au, int av, int bu, int bv, int i, int& j)
-{
-    const int cu = 256 * i + 128;
-    if (au != bu && min(au, bu) <= cu && cu <= max(au, bu))
-    {
-        // j = floor((av * den + (cu - au) * (bv - av) - 1) / (256 den)), den = bu - au made positive, through q, r of the product / den
-        long long n = (long long)(cu - au) * (long long)(bv - av), d = (long long)bu - au;
-        if (d < 0) n = -n, d = -d;
-        const long long q = floor_div64(n, d), r = n - q * d;
-        j                 = int(((long long)av + q - (r == 0 ? 1 : 0)) >> 8);
-    }
-    else
-    {
-        j = (av - 1) >> 8; // the start's diamond, if it lies in one
-        if (!in_diamond(au, av, cu, 256 * j + 128)) return false;
-    }
-    return !in_diamond(bu, bv, cu, 256 * j + 128); // the last-pixel rule: the segment must leave the diamond
 }
 
 DFX_HD bool covers(const BoxLine& L, int x, int y)

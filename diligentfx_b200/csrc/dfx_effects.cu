@@ -935,6 +935,8 @@ struct dfx_chain
     dfx_env_map_attribs   env{};
     bool                  box_on = false; // dfx_chain_set_bound_box
     dfx_bound_box_attribs box{};
+    float                 mv_elapsed = 0.0f; // dfx_chain_set_motion_vector_view (view_mode MOTION_VECTORS): the frame's ElapsedTime
+    PlaneOwner            mv_owner;          // the vector field's owner plane, all zero between frames
     dfx_chain_stats  stats{};
 
     void drop_graphs()
@@ -1027,7 +1029,10 @@ extern "C" dfx_status dfx_chain_set_config(dfx_chain* c, const dfx_chain_config*
         return set_error(DFX_ERR_INVALID_ARG, "disable_taa draws the frame in the final compose: the stage mask must include DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TONEMAP");
     if (c->sel_on && !config->disable_taa && (~config->stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TAA)))
         return set_error(DFX_ERR_INVALID_ARG, "the selection outline is drawn on the composed colour before TAA: a stage mask without DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TAA is refused while it is on");
-    if (debug_view(c->view_mode) && !config->disable_taa && (~config->stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TAA)))
+    if (c->view_mode == DFX_VIEW_MODE_MOTION_VECTORS && (~config->stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP)))
+        return set_error(DFX_ERR_INVALID_ARG, "the motion-vector view is drawn by the final compose: a stage mask without DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TONEMAP is refused while it is on");
+    if (debug_view(c->view_mode) && c->view_mode != DFX_VIEW_MODE_MOTION_VECTORS && !config->disable_taa &&
+        (~config->stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TAA)))
         return set_error(DFX_ERR_INVALID_ARG, "a debug view mode is drawn by the compose before TAA: a stage mask without DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TAA is refused while it is on");
     if (realloc || c->graphs.size() > 16)
     {
@@ -1075,7 +1080,8 @@ extern "C" dfx_status dfx_chain_set_view_mode(dfx_chain* c, int32_t view_mode, c
 {
     DFX_REQUIRE(c, "null argument");
     if (view_mode < 0 || view_mode >= DFX_VIEW_MODE_COUNT) return set_error(DFX_ERR_INVALID_ARG, "unknown view mode %d", view_mode);
-    if (view_mode == DFX_VIEW_MODE_MOTION_VECTORS) return set_error(DFX_ERR_UNSUPPORTED, "the motion-vector view (VectorFieldRenderer) is not built");
+    if (view_mode == DFX_VIEW_MODE_MOTION_VECTORS)
+        return set_error(DFX_ERR_UNSUPPORTED, "the motion-vector view takes the frame's elapsed time: use dfx_chain_set_motion_vector_view");
     if (debug_view(view_mode))
     {
         const uint32_t need = c->cfg.disable_taa ? DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP : DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TAA;
@@ -1132,6 +1138,21 @@ extern "C" dfx_status dfx_chain_set_bound_box(dfx_chain* c, const dfx_bound_box_
     c->box.Color[3] = 0.0f; // HnRenderBoundBoxTask's PS main: float4(Color.rgb, 0.0) (HnRenderBoundBoxTask.cpp:90)
     return DFX_OK;          // graphs are keyed on the attribs: the next frame records or replays the matching one
 }
+extern "C" dfx_status dfx_chain_set_motion_vector_view(dfx_chain* c, int32_t on, float elapsed_time)
+{
+    DFX_REQUIRE(c, "null argument");
+    if (!on)
+    {
+        if (c->view_mode == DFX_VIEW_MODE_MOTION_VECTORS) c->view_mode = DFX_VIEW_MODE_SHADED;
+        return DFX_OK;
+    }
+    DFX_REQUIRE(std::isfinite(elapsed_time), "elapsed_time must be finite");
+    DFX_REQUIRE(!(~c->cfg.stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP)),
+                "the motion-vector view is drawn by the final compose: the chain's stage mask lacks DFX_CHAIN_STAGE_COMPOSE or DFX_CHAIN_STAGE_TONEMAP");
+    c->view_mode = DFX_VIEW_MODE_MOTION_VECTORS, c->mesh_id = dfx_plane{}, c->loading_factor = 0.0f;
+    c->mv_elapsed = elapsed_time;
+    return DFX_OK; // graphs are keyed on the mode only: the elapsed time reaches the field's launches, which run after the graph
+}
 extern "C" dfx_status dfx_chain_get_config(const dfx_chain* c, dfx_chain_config* out)
 {
     DFX_REQUIRE(c && out, "null argument");
@@ -1184,6 +1205,7 @@ struct FrameCtx
     bool                   debug;                // a renderer debug view: no SSR, SSAO, Bloom or DoF
     bool                   env;                  // E draws the environment map into the frame's colour and motion first
     bool                   box;                  // B draws the bounding box into them next
+    bool                   mv;                   // the motion-vector view: F, then the vector field over ldr_out
 };
 
 // P0, then P1-P3 + S1 + S2 + A2 in one pass on `s`; SSR and SSAO Execute then skip S1 / S2 and A2
@@ -1299,7 +1321,8 @@ dfx_status record_front(const FrameCtx& x, cudaStream_t s, dfx_plane* color_out)
         }
         // F (HnPostProcess.psh drawn into the final target with TAA off): the grid reads the frame's depth and current camera
         else if (x.final_compose)
-            return dfx_pass_compose_final(s, c->pfx->cams_dev, &color, pssr, pao, cfg.ssr_scale, cfg.ssao_scale, &cfg.tonemap, cfg.ave_log_lum, cfg.to_srgb,
+            return dfx_pass_compose_final(s, c->pfx->cams_dev, &color, pssr, pao, x.mv ? 0.0f : cfg.ssr_scale, x.mv ? 0.0f : cfg.ssao_scale, &cfg.tonemap,
+                                          cfg.ave_log_lum, cfg.to_srgb,
                                           x.sel ? &x.sel_shader : nullptr, f->depth, &c->sel_depth, &c->sel_loc.p, c->grid_flags, &c->grid, f->ldr_out,
                                           dfx_rows{0, c->h});
         else if (!x.fuse_compose)
@@ -1364,8 +1387,10 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
     // With TAA off there is no TAA, hence no Bloom and no DepthOfField (HnPostProcessTask.cpp:652-654). A debug view mode runs no SSR,
     // SSAO, Bloom or DepthOfField (:625-654), and PostFX only where TAA runs (:788)
     const bool debug = debug_view(c->view_mode);
-    uint32_t   st    = cfg.disable_taa ? cfg.stages & ~(DFX_CHAIN_STAGE_TAA | DFX_CHAIN_STAGE_BLOOM) : cfg.stages;
-    if (debug) st &= ~(DFX_CHAIN_STAGE_SSR | DFX_CHAIN_STAGE_SSAO | DFX_CHAIN_STAGE_BLOOM | (cfg.disable_taa ? DFX_CHAIN_STAGE_POSTFX : 0u));
+    // The motion-vector view switches TAA off (:652) and with it PostFX (:788): F draws the frame, the vector field goes over it
+    const bool mv = c->view_mode == DFX_VIEW_MODE_MOTION_VECTORS;
+    uint32_t   st = cfg.disable_taa || mv ? cfg.stages & ~(DFX_CHAIN_STAGE_TAA | DFX_CHAIN_STAGE_BLOOM) : cfg.stages;
+    if (debug) st &= ~(DFX_CHAIN_STAGE_SSR | DFX_CHAIN_STAGE_SSAO | DFX_CHAIN_STAGE_BLOOM | (cfg.disable_taa || mv ? DFX_CHAIN_STAGE_POSTFX : 0u));
     DFX_REQUIRE(!(st & (DFX_CHAIN_STAGE_TONEMAP)) || f->ldr_out, "the tone-mapped output plane must be given");
     cudaStream_t main = as_stream(stream);
     FrameCtx     x{c, f, st, false, false, false, false, false, false, false, false, false, {}, false, debug};
@@ -1374,7 +1399,8 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
     x.grid          = c->grid_flags != 0;
     x.env           = c->env_on && c->view_mode != DFX_VIEW_MODE_SCENE_DEPTH; // HnRenderEnvMapTask::IsActive (HnRenderEnvMapTask.cpp:85-94)
     x.box           = c->box_on; // HnRenderBoundBoxTask has no IsActive: every view mode
-    x.final_compose = cfg.disable_taa != 0;
+    x.mv            = mv;
+    x.final_compose = cfg.disable_taa != 0 || mv;
     x.with_dof      = cfg.enable_dof != 0 && !x.final_compose && !debug;
     x.side_ao      = cfg.overlap && (st & DFX_CHAIN_STAGE_SSAO) && (st & DFX_CHAIN_STAGE_SSR);
     x.side_post    = cfg.overlap && (st & DFX_CHAIN_STAGE_BLOOM) && (st & DFX_CHAIN_STAGE_TAA) && !x.with_dof && !x.grid;
@@ -1413,6 +1439,11 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
     if ((st & DFX_CHAIN_STAGE_COMPOSE) && !x.fuse_compose && !x.final_compose && !c->composed.p.ptr && (s = c->composed.alloc(c->w, c->h, DFX_FORMAT_RGBA32F)) != DFX_OK) return s;
     for (PlaneOwner* p : {&c->sel_loc, &c->sel_scratch})
         if (x.sel && !p->p.ptr && (s = p->alloc(c->w, c->h, DFX_FORMAT_RG32F)) != DFX_OK) return s;
+    if (mv && !c->mv_owner.p.ptr)
+    {
+        if ((s = c->mv_owner.alloc(c->w, c->h, DFX_FORMAT_R32F)) != DFX_OK) return s;
+        DFX_CUDA(cudaMemsetAsync(c->mv_owner.p.ptr, 0, c->mv_owner.p.pitch_bytes * size_t(c->h), main));
+    }
     // the front pass needs every pass it replaces in this frame, at full resolution; dfx_tune "front_fused" = 0 keeps the separate passes
     const uint32_t front_stages = DFX_CHAIN_STAGE_POSTFX | DFX_CHAIN_STAGE_SSR | DFX_CHAIN_STAGE_SSAO;
     x.front = cfg.fuse && (st & front_stages) == front_stages && !(cfg.ssr_flags & DFX_SSR_FEATURE_FLAG_HALF_RESOLUTION) &&
@@ -1558,6 +1589,15 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
             DFX_CUDA(cudaStreamWaitEvent(main, c->post_done[par], 0));
             c->post_pending[par] = false;
         }
+    }
+    // the vector field over the final frame (HnPostProcessTask.cpp:928-943), outside the graph: its scale changes every frame
+    if (mv)
+    {
+        dfx_vector_field_attribs va;
+        dfx_vector_field_attribs_hydrogent(uint32_t(c->w), uint32_t(c->h), c->mv_elapsed, &va);
+        if ((s = dfx_pass_vector_field(main, &va, cfg.to_srgb ? DFX_VECTOR_FIELD_OPTION_CONVERT_OUTPUT_TO_SRGB : 0u, f->motion, f->ldr_out, &c->mv_owner.p,
+                                       dfx_rows{0, c->h})) != DFX_OK)
+            return s;
     }
     c->last_frame    = f->frame_index;
     c->sel_taa_reset = c->sel_taa_reset && !(st & DFX_CHAIN_STAGE_TAA);

@@ -618,3 +618,48 @@ def sphere_bound_box(k: int, seed: int = 7, count: int = 24) -> np.ndarray:
     scene = make_scene(seed, count)
     c, r = scene.centers[k], scene.radii[k]
     return bound_box_transform(c - r, c + r)
+
+
+# ---- motion fields for the vector field overlay (VectorFieldRenderer): (H, W, 2) float32 in the G-buffer's units, the NDC offset from the
+# previous to the current position of a pixel (GetMotionVector); -0.02 / elapsed scales them to the drawn vectors' NDC length
+
+def motion_pan(width: int, height: int, dx: float = 0.004, dy: float = -0.002) -> np.ndarray:
+    """A camera pan: the same motion everywhere."""
+    out = np.empty((height, width, 2), np.float32)
+    out[..., 0], out[..., 1] = np.float32(dx), np.float32(dy)
+    return out
+
+
+def _ndc_grid(width: int, height: int) -> tuple[np.ndarray, np.ndarray]:
+    x = (np.arange(width, dtype=np.float64) + 0.5) / width * 2.0 - 1.0
+    y = 1.0 - (np.arange(height, dtype=np.float64) + 0.5) / height * 2.0
+    return np.meshgrid(x, y)
+
+
+def motion_rotation(width: int, height: int, angle: float = 0.01) -> np.ndarray:
+    """A roll of the camera by `angle` radians about the frame's centre: motion proportional to the distance from it."""
+    X, Y = _ndc_grid(width, height)
+    c, s = np.cos(angle), np.sin(angle)
+    return np.stack([X - (c * X + s * Y), Y - (-s * X + c * Y)], -1).astype(np.float32)
+
+
+def motion_vortex(width: int, height: int, strength: float = 0.02, swirl: float = 0.5) -> np.ndarray:
+    """A converging vortex: every vector points past the centre and turns about it, so many lines cross there (heavy overlap)."""
+    X, Y = _ndc_grid(width, height)
+    return np.stack([strength * (X - swirl * Y), strength * (Y + swirl * X)], -1).astype(np.float32)
+
+
+def motion_random(width: int, height: int, seed: int = 0, sigma: float = 0.01) -> np.ndarray:
+    """Independent Gaussian motion per pixel."""
+    return np.random.default_rng(seed).normal(0.0, sigma, (height, width, 2)).astype(np.float32)
+
+
+def motion_extreme(width: int, height: int, seed: int = 0) -> np.ndarray:
+    """Random motion with the values a renderer must not produce but a field may hold: NaN, +-Inf, the largest floats, denormals, and
+    vectors long enough to put a line's end beyond the 2^20-pixel guard band."""
+    rng = np.random.default_rng(seed)
+    out = rng.normal(0.0, 0.05, (height, width, 2)).astype(np.float32)
+    special = np.array([np.nan, np.inf, -np.inf, 3.4e38, -3.4e38, 1e-45, 1e4, -1e4, 0.0], np.float32)
+    pick = rng.random((height, width, 2)) < 0.3
+    out[pick] = special[rng.integers(0, len(special), int(pick.sum()))]
+    return out

@@ -305,6 +305,21 @@ typedef struct dfx_bound_box_attribs
 #define DFX_BOUND_BOX_OPTION_USE_REVERSE_DEPTH      (1u << 2)
 #define DFX_BOUND_BOX_OPTION_ALL                    7u
 
+/* VectorFieldRenderer::RenderAttribs' values (Components/interface/VectorFieldRenderer.hpp), what Render (VectorFieldRenderer.cpp:173-223)
+ * writes into VectorField.vsh's constant block: ScaleAndBias = (Scale, Bias), the grid size as float and as uint, the two colours. */
+typedef struct dfx_vector_field_attribs
+{
+    float    Bias[2];       /* (0, 0): added to the field's value first                         */
+    float    Scale[2];      /* (1, 1): then multiplied, in NDC units                              */
+    float    StartColor[4]; /* (1, 1, 1, 1): the colour at the cell's centre                      */
+    float    EndColor[4];   /* (1, 1, 1, 1): the colour at the vector's end                       */
+    uint32_t GridSize[2];   /* (0, 0): lines across and down; 0 in either draws nothing           */
+} dfx_vector_field_attribs;
+/* VectorFieldRenderer::RenderAttribs::ConvertOutputToSRGB */
+#define DFX_VECTOR_FIELD_OPTION_NONE                   0u
+#define DFX_VECTOR_FIELD_OPTION_CONVERT_OUTPUT_TO_SRGB (1u << 0)
+#define DFX_VECTOR_FIELD_OPTION_ALL                    1u
+
 /* Default-initialisers (the reference's DEFAULT_VALUE()s). */
 DFX_API void dfx_ssao_attribs_default(dfx_ssao_attribs* a);
 DFX_API void dfx_ssr_attribs_default(dfx_ssr_attribs* a);
@@ -318,6 +333,12 @@ DFX_API void dfx_selection_attribs_default(dfx_selection_attribs* a);
 DFX_API void dfx_env_map_attribs_default(dfx_env_map_attribs* a);
 /* BoundBoxRenderer::RenderAttribs' defaults: the identity transform, Color (1, 1, 1, 1), PatternLength 32, PatternMask 0xFFFFFFFF */
 DFX_API void dfx_bound_box_attribs_default(dfx_bound_box_attribs* a);
+/* VectorFieldRenderer::RenderAttribs' defaults: Bias (0, 0), Scale (1, 1), both colours (1, 1, 1, 1), GridSize (0, 0) */
+DFX_API void dfx_vector_field_attribs_default(dfx_vector_field_attribs* a);
+/* The attribs HnPostProcessTask draws the motion-vector view with (Hydrogent/src/Tasks/HnPostProcessTask.cpp:932-938) over a
+ * width x height final target: GridSize (width / 20, height / 20), Scale -0.02 / max(elapsed_time, 0.001) in both axes (the vectors
+ * point against the motion), StartColor (1, 1, 1, 1), EndColor (0.5, 0.5, 0.5, 1), Bias 0. */
+DFX_API void dfx_vector_field_attribs_hydrogent(uint32_t width, uint32_t height, float elapsed_time, dfx_vector_field_attribs* a);
 
 /* == PostFXContext::FrameDesc, PostProcess/Common/interface/PostFXContext.hpp:68-84 */
 typedef struct dfx_frame_desc
@@ -715,6 +736,21 @@ DFX_API dfx_status dfx_pass_env_map(void* stream, const dfx_camera_attribs* came
  * and > 0. */
 DFX_API dfx_status dfx_pass_bound_box(void* stream, const dfx_camera_attribs* cameras_dev, const dfx_bound_box_attribs* attribs, uint32_t options,
                                       const dfx_plane* depth, const dfx_plane* color_inout, const dfx_plane* motion_inout, dfx_rows rows);
+
+/* The vector field overlay (Components/src/VectorFieldRenderer.cpp:142-157 GetPSO, :173-223 Render; Shaders/Common/private/
+ * VectorField.vsh; the default PS main, :76-86), drawn over color_inout. Line k = row * GridSize.x + col runs from
+ * TexUVToNormalizedDeviceXY(UV), UV = ((col + 0.5) / GridSize.x, (row + 0.5) / GridSize.y), to that point plus
+ * (SampleLevel(vector_field, UV).xy + Bias) * Scale (a bilinear, clamped tap), at z = 0, w = 1, and is rasterised by the aliased-line
+ * rule of DESIGN.md §2 in the target-sized viewport: never clipped; a non-finite or far end (beyond the guard band) draws nothing.
+ * Its colour goes from StartColor to EndColor through the rule's perspective-correct t; with
+ * DFX_VECTOR_FIELD_OPTION_CONVERT_OUTPUT_TO_SRGB rgb becomes pow(rgb, 1 / 2.2). No depth test and no blending: a pixel several lines
+ * cover takes the last line's fragment in primitive order (the highest k); every other pixel is not touched. vector_field RG32F or
+ * RG16F, any size; color_inout RGBA32F or RGBA16F (the 16-bit stores round to nearest even); scratch an R32F plane of the target's
+ * size whose texels are read as 32-bit words: all zero on entry, and left all zero. Any row range; only its rows are touched, and
+ * they are the rows of a full call. Two launches, no host synchronisation. Refuses unknown option bits, bad or mismatched planes and
+ * a GridSize whose vertex count 2 * GridSize.x * GridSize.y does not fit in 32 bits. */
+DFX_API dfx_status dfx_pass_vector_field(void* stream, const dfx_vector_field_attribs* attribs, uint32_t options, const dfx_plane* vector_field,
+                                         const dfx_plane* color_inout, const dfx_plane* scratch, dfx_rows rows);
 
 /* J the closest selected location (Hydrogent/src/Tasks/HnProcessSelectionTask.cpp:304-369): HnInitClosestSelectedLocation.psh on
  * `selection_depth` (R32F; a texel != clear_depth is selected), then dfx_selection_jfa_iterations(max_distance) steps of
@@ -1168,7 +1204,8 @@ DFX_API dfx_status dfx_chain_set_selection(dfx_chain* chain, const dfx_selection
  *   step). With disable_taa it writes ldr_out with the tone map, the selection colours as given, the grid and sRGB.
  * A switch does not reset TAA. mesh_id: R32F, the chain's size, read by every MESH_ID frame (it must stay valid while that mode is
  * on); ignored by the other modes. loading_animation_factor: g_Frame.Renderer.LoadingAnimation.Factor, read by SCENE_DEPTH (non-zero
- * skips the rescale). Refuses an unknown mode, MOTION_VECTORS (DFX_ERR_UNSUPPORTED: VectorFieldRenderer is not built), MESH_ID
+ * skips the rescale). Refuses an unknown mode, MOTION_VECTORS (DFX_ERR_UNSUPPORTED: that view takes the frame's elapsed time, through
+ * dfx_chain_set_motion_vector_view), MESH_ID
  * without a chain-sized R32F plane, and a debug view when the stages lack COMPOSE + TAA (or COMPOSE + TONEMAP with disable_taa);
  * dfx_chain_set_config refuses such stages while a debug view is on. */
 DFX_API dfx_status dfx_chain_set_view_mode(dfx_chain* chain, int32_t view_mode, const dfx_plane* mesh_id, float loading_animation_factor);
@@ -1190,6 +1227,18 @@ DFX_API dfx_status dfx_chain_set_environment_map(dfx_chain* chain, int32_t type,
  * attribs NULL switches B off (the default): the chain then issues exactly the kernels it issues without it. Refuses a PatternLength
  * that is not finite and > 0. */
 DFX_API dfx_status dfx_chain_set_bound_box(dfx_chain* chain, const dfx_bound_box_attribs* attribs);
+/* The motion-vector view (HN_VIEW_MODE_MOTION_VECTORS; HnPostProcessTask.cpp:625-654, :788, :928-943): on != 0 makes every following
+ * frame (replayed frames included) run E and B when they are on, J when the selection is on, then F (dfx_pass_compose_final) into
+ * ldr_out with zero SSR and SSAO scales, the configured tone map, the selection colours as given, the grid and sRGB, and then the
+ * vector field of the frame's motion plane over ldr_out (dfx_pass_vector_field with dfx_vector_field_attribs_hydrogent(width, height,
+ * elapsed_time), sRGB = to_srgb), whatever disable_taa says: no PostFX, SSR, SSAO, TAA, Bloom or DepthOfField. elapsed_time is the
+ * frame's ElapsedTime in seconds; call again with the next frame's before each frame. The field's two launches are issued after the
+ * frame's graph on the caller's stream, so a new elapsed time replays the same graph. The first frame allocates a chain-sized scratch
+ * plane. on = 0 leaves the view for SHADED (nothing changes when the view is off); dfx_chain_set_view_mode with any mode leaves it too.
+ * The first TAA frame after motion-vector frames resets TAA's history (the frame indices are not consecutive). Refuses a non-finite
+ * elapsed_time and, with on != 0, a stage mask without COMPOSE + TONEMAP; dfx_chain_set_config refuses such masks while the view is
+ * on. */
+DFX_API dfx_status dfx_chain_set_motion_vector_view(dfx_chain* chain, int32_t on, float elapsed_time);
 
 /* ============================================================================================================ */
 /* 4. one frame split into row strips over the GPUs of a box (no reference counterpart)                          */

@@ -8,6 +8,7 @@ RGBA8 results are written as .npy (or .ppm with --ppm).
     python tools/run_chain.py --in /tmp/seq --out /tmp/seq_ldr                                      # on the GPU
     python tools/run_chain.py --in /tmp/seq --out /tmp/seq_grid --grid 126                          # ... with the coordinate grid and axes
     python tools/run_chain.py --in /tmp/seq --out /tmp/seq_notaa --no-taa                           # ... as a viewer with TAA off draws it
+    python tools/run_chain.py --in /tmp/seq --out /tmp/seq_mv --view-mode motion-vectors            # ... the motion-vector view at 60 fps
 """
 import argparse
 import os
@@ -19,7 +20,7 @@ import torch  # noqa: E402
 from diligentfx_b200 import gbuffer_io, synth  # noqa: E402
 
 ap = argparse.ArgumentParser()
-VIEW_MODES = {"shaded": 0, "scene-depth": 24, "edge-map": 25, "mesh-id": 26}  # HN_VIEW_MODE (capi.VIEW_MODE_*)
+VIEW_MODES = {"shaded": 0, "motion-vectors": 14, "scene-depth": 24, "edge-map": 25, "mesh-id": 26}  # HN_VIEW_MODE (capi.VIEW_MODE_*)
 ap.add_argument("--width", type=int, default=3840)
 ap.add_argument("--height", type=int, default=2160)
 ap.add_argument("--frames", type=int, default=3)
@@ -34,7 +35,8 @@ ap.add_argument("--no-taa", action="store_true",
                 help="the frame of HnPostProcessTask with EnableTAA = false: no TAA, no Bloom, the final compose draws tone map, grid and sRGB")
 ap.add_argument("--view-mode", choices=sorted(VIEW_MODES), default="shaded",
                 help="the viewer's view mode: scene-depth (the colour is the renderer's scene-depth view), edge-map or mesh-id (the synthetic "
-                     "sequence's mesh IDs; frame files carry no mesh-ID plane)")
+                     "sequence's mesh IDs; frame files carry no mesh-ID plane) or motion-vectors (the frame's motion drawn as lines over it)")
+ap.add_argument("--elapsed", type=float, default=1 / 60, help="motion-vectors: the seconds between frames, which scale the lines (default 1/60)")
 a = ap.parse_args()
 
 if a.write_synthetic:
@@ -45,6 +47,14 @@ if a.write_synthetic:
     sys.exit(0)
 
 from diligentfx_b200.chain import ChainConfig, PostProcessChain  # noqa: E402  (loads the CUDA library: fails loudly without it)
+
+
+def set_view(chain, ids=None):
+    if a.view_mode == "motion-vectors":
+        chain.set_motion_vector_view(a.elapsed)
+    else:
+        chain.set_view_mode(VIEW_MODES[a.view_mode], ids)
+
 
 cfg = ChainConfig(enable_taa=not a.no_taa)
 
@@ -61,7 +71,7 @@ if a.src:
     h, w = first["depth"].shape
     chain = PostProcessChain(w, h, cfg)
     chain.set_coordinate_grid(a.grid)
-    chain.set_view_mode(VIEW_MODES[a.view_mode])
+    set_view(chain)
     results = [torch.empty((h, w, 4), dtype=torch.uint8).pin_memory() for _ in range(a.batch)]
     done = 0
     for b0 in range(0, len(paths), a.batch):
@@ -79,7 +89,7 @@ else:
     chain = PostProcessChain(a.width, a.height, cfg)
     chain.set_coordinate_grid(a.grid)
     ids = torch.empty((a.height, a.width), dtype=torch.float32, device="cuda")
-    chain.set_view_mode(VIEW_MODES[a.view_mode], ids)
+    set_view(chain, ids)
     for fr in seq:
         if a.view_mode == "scene-depth":
             fr = dict(fr, color=synth.scene_depth_colour(fr))
