@@ -148,6 +148,12 @@ class EnvMapAttribs(C.Structure):
 ENV_MAP_TYPE_CUBE, ENV_MAP_TYPE_SPHERE = 0, 1
 ENV_MAP_OPTION_CONVERT_OUTPUT_TO_SRGB, ENV_MAP_OPTION_COMPUTE_MOTION_VECTORS, ENV_MAP_OPTION_USE_REVERSE_DEPTH = 1, 2, 4
 
+# IBL cube-map precomputation (dfx_pass_irradiance_cube / dfx_pass_prefilter_env_map): the most levels of a source map or output chain,
+# and PBR_Renderer's defaults (PBR/interface/PBR_Renderer.hpp: IrradianceCubeDim, PrefilteredEnvMapDim; the sample counts 0 stands for)
+MAX_ENV_LEVELS = 16
+IRRADIANCE_CUBE_DIM, PREFILTERED_ENV_MAP_DIM = 64, 256
+DEFAULT_DIFFUSE_SAMPLES, DEFAULT_SPECULAR_SAMPLES = 8192, 256
+
 
 class BoundBoxAttribs(C.Structure):
     """dfx_bound_box_attribs == BoundBoxAttribs (BoundBoxStructures.fxh, 96 bytes). Transform is row-major, row-vector convention."""

@@ -719,6 +719,34 @@ DFX_API dfx_status dfx_pass_env_map(void* stream, const dfx_camera_attribs* came
                                     uint32_t options, const dfx_env_map_attribs* attribs, const dfx_plane* depth,
                                     const dfx_plane* color_inout, const dfx_plane* motion_inout, dfx_rows rows);
 
+/* The most levels an IBL source map or output chain may have (a 32768^2 map's full chain; a 2048^2 HDRI has 12). */
+#define DFX_MAX_ENV_LEVELS 16
+/* IBL cube-map precomputation (PBR/src/PBR_Renderer.cpp:729-970 PrecomputeCubemaps): the image-based-lighting cubes a PBR renderer
+ * samples, convolved from an environment map. Both passes draw every texel of every face of their output with the texel direction
+ * N = normalize(CubemapFace.vsh at the pixel centre: g_Rotation[face] * (x, y, 1, 1), x = 2(i + 1/2)/s - 1, y = 1 - 2(j + 1/2)/s),
+ * through the face matrices of PBR_Renderer.cpp:913-922 as float values (DESIGN.md §2), and sample the source with E's sampler
+ * (Sam_LinearClamp: trilinear, the seamless cube rule of DESIGN.md §2). Each sample is the reference shader's arithmetic, one rounding
+ * per operation, transcendentals correctly rounded; the samples of a texel are summed in another order than the shader's, within
+ * the bound DESIGN.md §2 derives.
+ *   env_type   DFX_ENV_MAP_TYPE_CUBE (level i is s_i x 6 s_i, faces +X, -X, +Y, -Y, +Z, -Z stacked) or DFX_ENV_MAP_TYPE_SPHERE
+ *              (a lat-long map w_i x h_i); env_levels[0..n_env) its mip chain, level i max(w0 >> i, 1) x max(h0 >> i, 1) (cube:
+ *              s_i = max(s0 >> i, 1)), 1 <= n_env <= DFX_MAX_ENV_LEVELS, RGBA32F or RGBA16F, one format for all levels. g_EnvMipCount
+ *              is n_env; g_EnvMapWidth / Height are level 0's face size (cube) or w0 x h0 (sphere).
+ *   num_samples 0 = the reference default: 8192 for the irradiance (GetDefaultDiffuseSamplesCount on a discrete adapter), 256 for
+ *              the prefilter.
+ *   optimize_samples  OPTIMIZE_SAMPLES: 1 picks each sample's LOD from its solid angle (mip bias 1), 0 reads level 0.
+ *   outputs    cube planes s x 6s, RGBA16F (IrradianceCubeFmt / PrefilteredEnvMapFmt) or RGBA32F, stored rounded to nearest even.
+ * Nothing else is read or written; the work is enqueued on `stream` without host synchronisation.                                */
+/* ComputeIrradianceMap.psh: rgb = the mean of SampleLevel(L_k) over the cosine-weighted directions L_k around N, alpha 1. */
+DFX_API dfx_status dfx_pass_irradiance_cube(void* stream, int32_t env_type, const dfx_plane* env_levels, int32_t n_env,
+                                            uint32_t num_samples, int32_t optimize_samples, const dfx_plane* out);
+/* PrefilterEnvMap.psh: out_levels[0..n_out) is a chain (level m is max(s0 >> m, 1) x 6 of that, one format, 2 <= n_out <=
+ * DFX_MAX_ENV_LEVELS) and level m is prefiltered at PerceptualRoughness m / (n_out - 1) (PBR_Renderer.cpp:951): rgb =
+ * sum(SampleLevel(L_k) * NoL_k) / sum(NoL_k) over the GGX-importance-sampled reflections L_k of R = N, alpha 0. All levels are
+ * written by one launch. n_out = 1 is refused: the reference divides 0 by 0 there. */
+DFX_API dfx_status dfx_pass_prefilter_env_map(void* stream, int32_t env_type, const dfx_plane* env_levels, int32_t n_env,
+                                              uint32_t num_samples, int32_t optimize_samples, const dfx_plane* out_levels, int32_t n_out);
+
 /* B the selected prim's bounding box (Components/src/BoundBoxRenderer.cpp:150-168 GetPSO, :257-277 Render; Shaders/Common/private/
  * BoundBox.vsh, BoundBox.psh:27-48 GetBoundBoxOutput), in place on the G-buffer's colour and motion planes. The 24 vertices of
  * BoundBoxVS (GetBoxCorner's table through attribs->Transform, then cameras_dev[0].mViewProj; PREV_CLIP_POS through cameras_dev[1]'s)
