@@ -14,12 +14,14 @@
 // launch: a CTA finds its level from the per-level CTA offsets.
 #include "dfx_common.cuh"
 #include "dfx_env_sample.cuh"
+#include "dfx_ibl_math.cuh"
 
 namespace dfx
 {
 namespace
 {
 using namespace envs;
+using namespace iblm;
 
 constexpr int kWarps = 8, kThreads = 32 * kWarps, kChunk = kThreads; // samples staged per CTA and round
 
@@ -35,45 +37,9 @@ __constant__ float kFaceRot[6][3][4] = {
     {{-1.0f, 0.0f, -kS180, 0.0f}, {0.0f, 1.0f, 0.0f, 0.0f}, {kS180, 0.0f, -1.0f, 0.0f}}, // -Z RotationY(-pi)
 };
 
-// correctly rounded transcendentals: the double result rounded once. cos / sin go through cospi / sinpi of x / pi (a double relative
-// error of a few 2^-53 for the arguments here, 2 pi Xi.x in [0, 2 pi) and the sphere's theta -+ dtheta / 2 just outside [0, pi]); double
-// cos / sin would pull in the Payne-Hanek slow path's stack frame.
-DFX_HD float cos_(float x) { return float(cospi(double(x) * 0.31830988618379067)); }
-DFX_HD float sin_(float x) { return float(sinpi(double(x) * 0.31830988618379067)); }
+// acos / log2 correctly rounded (the double result rounded once); cos_, sin_, sqrt_ and the vector helpers are dfx_ibl_math.cuh's
 DFX_HD float acos_(float x) { return float(acos(double(x))); }
 DFX_HD float log2_(float x) { return float(log2(double(x))); }
-// sqrt(a) correctly rounded without sqrt.rn.f32's slow-path call (the call makes the kernels spill): a double reciprocal square root
-// estimate, two Newton steps and one correction give sqrt(a) within a few 2^-53; the square root of a float is never that close to a
-// float rounding midpoint, so rounding it to float is the correctly rounded result. Float denormals are normal doubles.
-DFX_HD float sqrt_(float a)
-{
-    if (!(a > 0.0f && a <= kFltMax)) return a == 0.0f || a > kFltMax ? a : __int_as_float(0x7fffffff); // +-0, +inf; NaN for a < 0 or NaN
-    const double d = a;
-    double       y;
-    asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(d));
-    const double h = 0.5 * d;
-    y              = y * fma(-h * y, y, 1.5);
-    y              = y * fma(-h * y, y, 1.5);
-    const double r = d * y;
-    return float(fma(fma(-r, r, d), 0.5 * y, r));
-}
-DFX_HD float sat_(float x) { return fminf(fmaxf(x, 0.0f), 1.0f); } // saturate: NaN -> 0
-DFX_HD float dot3(float3 a, float3 b) { return add_(add_(mul_(a.x, b.x), mul_(a.y, b.y)), mul_(a.z, b.z)); }
-DFX_HD float3 normalize3(float3 a)
-{
-    const float l = sqrt_(dot3(a, a));
-    return make_float3(div_(a.x, l), div_(a.y, l), div_(a.z, l));
-}
-DFX_HD float3 cross3(float3 a, float3 b)
-{
-    return make_float3(sub_(mul_(a.y, b.z), mul_(a.z, b.y)), sub_(mul_(a.z, b.x), mul_(a.x, b.z)), sub_(mul_(a.x, b.y), mul_(a.y, b.x)));
-}
-// a * x + b * y + c * z per component: ((a.c * x + b.c * y) + c.c * z)
-DFX_HD float3 combine3(float3 a, float x, float3 b, float y, float3 c, float z)
-{
-    return make_float3(add_(add_(mul_(a.x, x), mul_(b.x, y)), mul_(c.x, z)), add_(add_(mul_(a.y, x), mul_(b.y, y)), mul_(c.y, z)),
-                       add_(add_(mul_(a.z, x), mul_(b.z, y)), mul_(c.z, z)));
-}
 
 // normalize(WorldPos) of CubemapFace.vsh at the centre of texel (i, j) of face f of an s x s face: mul(g_Rotation, (x, y, 1, 1)), xyz / w
 DFX_HD float3 texel_dir(int f, int i, int j, int s)
@@ -86,9 +52,6 @@ DFX_HD float3 texel_dir(int f, int i, int j, int s)
     // row 3 is (0, 0, 0, 1): w = ((0 * x + 0 * y) + 0) + 1 = 1 exactly
     return normalize3(make_float3(div_(w[0], 1.0f), div_(w[1], 1.0f), div_(w[2], 1.0f)));
 }
-
-// Hammersley2D (PBR_PrecomputeCommon.fxh:10-16)
-DFX_HD float2 hammersley(uint32_t i, uint32_t n) { return make_float2(div_(float(i), float(n)), mul_(__uint2float_rn(__brev(i)), 2.3283064365386963e-10f)); }
 
 // ComputeSphereMapPixelSolidAngle (PBR_PrecomputeCommon.fxh:43-48), the reference's dTheta = PI / Width, dPhi = 2 PI / Height
 DFX_HD float sphere_pixel_solid_angle(float w, float h, float theta, float gamma)

@@ -91,7 +91,7 @@ float2 taa_jitter_offset(uint frame_index, uint width, uint height); // Temporal
 void compose(const TexF4& color, const TexF4* ssr, const TexF* ao, float ssr_scale, float ssao_scale, TexF4& out, int threads);
 // Full form (Hydrogent/shaders/HnPostProcess.psh:145-185): SSR re-weighted by the split-sum BRDF and exchanged for the specular
 // IBL it replaces, both scaled by the pixel's opacity. `lut` = brdf_lut() (PrecomputeBRDF.psh:10-48). oracle_compose_ibl.cpp
-void brdf_lut(int size, uint num_samples, TexF2& lut, int threads);
+void brdf_lut(int w, int h, uint num_samples, TexF2& lut, int threads);
 void compose_ibl(const Camera& cam, const TexF4& color, const TexF4* ssr, const TexF* ao, const TexF4& specular_ibl, const TexF4& normal,
                  const TexF4& base_color, const TexF4& material, const TexF2& lut, float ssr_scale, float ssao_scale, TexF4& out, int threads);
 

@@ -559,10 +559,10 @@ ORC_API void     orc_taa_jitter(uint32_t frame, uint32_t w, uint32_t hgt, float*
     float2 j = taa_jitter_offset(frame, w, hgt);
     out[0] = j.x, out[1] = j.y;
 }
-ORC_API void orc_brdf_lut(void* h, int size, uint32_t num_samples)
+ORC_API void orc_brdf_lut(void* h, int w, int hgt, uint32_t num_samples)
 {
     Ctx& c = *static_cast<Ctx*>(h);
-    orc::brdf_lut(size, num_samples, c.f2["brdf_lut"], c.threads);
+    orc::brdf_lut(w, hgt, num_samples, c.f2["brdf_lut"], c.threads);
 }
 ORC_API void orc_set_reversed_depth(int on) { orc::g_reversed_depth = on != 0; } // process-wide, like a shader macro
 ORC_API void orc_march_stats(unsigned long long* rays, unsigned long long* iterations, int reset)

@@ -4,44 +4,13 @@
 // :86-95) and the pre-integrated GGX look-up table those helpers sample (Shaders/PBR/private/PrecomputeBRDF.psh:10-48,
 // PBR_PrecomputeCommon.fxh:10-39; created 512x512 RG16_FLOAT with 512 samples by PBR/src/PBR_Renderer.cpp:548-625).
 #include "oracle.h"
+#include "oracle_ibl_math.h"
 
 namespace orc
 {
 
-static inline uint reversebits(uint v)
-{
-    v = ((v >> 1) & 0x55555555u) | ((v & 0x55555555u) << 1);
-    v = ((v >> 2) & 0x33333333u) | ((v & 0x33333333u) << 2);
-    v = ((v >> 4) & 0x0F0F0F0Fu) | ((v & 0x0F0F0F0Fu) << 4);
-    v = ((v >> 8) & 0x00FF00FFu) | ((v & 0x00FF00FFu) << 8);
-    return (v >> 16) | (v << 16);
-}
-
-// PBR_PrecomputeCommon.fxh:10-16
-static inline float2 Hammersley2D(uint i, uint N)
-{
-    uint  bits = reversebits(i);
-    float rdi  = float(bits) * 2.3283064365386963e-10f;
-    return float2(float(i) / float(N), rdi);
-}
-
-// PBR_PrecomputeCommon.fxh:19-39
-static inline float3 ImportanceSampleGGX(float2 Xi, float PerceptualRoughness, float3 N)
-{
-    const float PI_ = 3.141592653589793f;
-    float AlphaRoughness = PerceptualRoughness * PerceptualRoughness;
-    float a2             = AlphaRoughness * AlphaRoughness;
-    float Phi            = 2.0f * PI_ * Xi.x;
-    float CosTheta       = std::sqrt(saturate((1.0f - Xi.y) / (1.0f + (a2 - 1.0f) * Xi.y)));
-    float SinTheta       = std::sqrt(saturate(1.0f - CosTheta * CosTheta));
-    float3 H(SinTheta * std::cos(Phi), SinTheta * std::sin(Phi), CosTheta);
-    float3 UpVector = std::fabs(N.z) < 0.999f ? float3(0.0f, 0.0f, 1.0f) : float3(1.0f, 0.0f, 0.0f);
-    float3 TangentX = normalize(cross(UpVector, N));
-    float3 TangentY = cross(N, TangentX);
-    return TangentX * H.x + TangentY * H.y + N * H.z;
-}
-
-// PrecomputeBRDF.psh:10-38
+// PrecomputeBRDF.psh:10-38 under DESIGN.md §2's rule for PBR_Renderer's precomputations (oracle_ibl_math.h): one rounding per
+// operation, cos / sin correctly rounded, pow(1 - VoH, 5.0) as pow5_; the samples are added in order
 static float2 IntegrateBRDF(float PerceptualRoughness, float NoV, uint NumSamples)
 {
     float3 V(std::sqrt(1.0f - NoV * NoV), 0.0f, NoV);
@@ -49,15 +18,15 @@ static float2 IntegrateBRDF(float PerceptualRoughness, float NoV, uint NumSample
     float A = 0.0f, B = 0.0f;
     for (uint i = 0u; i < NumSamples; i++)
     {
-        float2 Xi  = Hammersley2D(i, NumSamples);
-        float3 H   = ImportanceSampleGGX(Xi, PerceptualRoughness, N);
+        float2 Xi  = iblm::hammersley(i, NumSamples);
+        float3 H   = iblm::ImportanceSampleGGX(Xi, PerceptualRoughness, N);
         float3 L   = 2.0f * dot(V, H) * H - V;
         float  NoL = saturate(L.z), NoH = saturate(H.z), VoH = saturate(dot(V, H));
         if (NoL > 0.0f)
         {
             float AlphaRoughness = PerceptualRoughness * PerceptualRoughness;
             float G_Vis = 4.0f * SmithGGXVisibilityCorrelated(NoL, NoV, AlphaRoughness) * VoH * NoL / NoH;
-            float Fc    = std::pow(1.0f - VoH, 5.0f);
+            float Fc    = iblm::pow5_(1.0f - VoH);
             A += (1.0f - Fc) * G_Vis;
             B += Fc * G_Vis;
         }
@@ -65,15 +34,15 @@ static float2 IntegrateBRDF(float PerceptualRoughness, float NoV, uint NumSample
     return float2(A, B) / float(NumSamples);
 }
 
-// PrecomputeBRDF.psh:40-48: texel (x, y) holds IntegrateBRDF(roughness = v, NdotV = u) at its centre
-void brdf_lut(int size, uint num_samples, TexF2& lut, int threads)
+// PrecomputeBRDF.psh:40-48: texel (x, y) of a w x h table holds IntegrateBRDF(roughness = v, NdotV = u) at its centre
+void brdf_lut(int w, int h, uint num_samples, TexF2& lut, int threads)
 {
-    lut.resize(size, size);
-    parallel_rows(0, size, threads, [&](int ya, int yb) {
+    lut.resize(w, h);
+    parallel_rows(0, h, threads, [&](int ya, int yb) {
         for (int y = ya; y < yb; ++y)
-            for (int x = 0; x < size; ++x)
+            for (int x = 0; x < w; ++x)
             {
-                float2 UV((float(x) + 0.5f) / float(size), (float(y) + 0.5f) / float(size));
+                float2 UV((float(x) + 0.5f) / float(w), (float(y) + 0.5f) / float(h));
                 lut.at(x, y) = IntegrateBRDF(UV.y, UV.x, num_samples);
             }
     });

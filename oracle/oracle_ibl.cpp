@@ -8,7 +8,7 @@
 // states it for E: trilinear, bilinear positions snapped to 1/256 texel, the seamless cube rule. Every transcendental (cos, sin, acos,
 // log2, and atan2 / asin of the sphere lookup) is the double function rounded once to float: DESIGN.md §2's statement of the HLSL intrinsics for these passes, which
 // the reference-shader build follows too (oracle/refshader/ibl_defs.inc).
-#include "oracle_math.h"
+#include "oracle_ibl_math.h"
 
 #include <algorithm>
 #include <cmath>
@@ -21,10 +21,8 @@ namespace orc
 {
 namespace
 {
-constexpr float kPi = 3.141592653589793f; // PBR_Common.fxh:5, the PI the include order leaves in force
+using namespace iblm; // kPi, cos_, sin_, hammersley, ImportanceSampleGGX
 
-float cos_(float x) { return float(std::cos(double(x))); }
-float sin_(float x) { return float(std::sin(double(x))); }
 float acos_(float x) { return float(std::acos(double(x))); }
 float log2_(float x) { return float(std::log2(double(x))); }
 
@@ -158,17 +156,6 @@ float3 texel_dir(int f, int i, int j, int s)
     return normalize(float3(w[0], w[1], w[2]) / w[3]);
 }
 
-float2 hammersley(uint32_t i, uint32_t n)
-{
-    uint32_t v = i;
-    v          = ((v >> 1) & 0x55555555u) | ((v & 0x55555555u) << 1);
-    v          = ((v >> 2) & 0x33333333u) | ((v & 0x33333333u) << 2);
-    v          = ((v >> 4) & 0x0F0F0F0Fu) | ((v & 0x0F0F0F0Fu) << 4);
-    v          = ((v >> 8) & 0x00FF00FFu) | ((v & 0x00FF00FFu) << 8);
-    v          = (v >> 16) | (v << 16);
-    return float2(float(i) / float(n), float(v) * 2.3283064365386963e-10f);
-}
-
 struct Source
 {
     std::vector<Level> M;
@@ -212,18 +199,11 @@ float3 prefilter(const Source& S, float rough, float3 R, uint32_t n, bool opt)
 {
     const float3 N = R, V = R;
     const float  alpha = rough * rough, a2 = alpha * alpha;
-    const float3 up = std::fabs(N.z) < 0.999f ? float3(0.0f, 0.0f, 1.0f) : float3(1.0f, 0.0f, 0.0f);
-    const float3 TX = normalize(cross(up, N)), TY = cross(N, TX);
     float3       acc(0.0f, 0.0f, 0.0f);
     float        total = 0.0f;
     for (uint32_t i = 0; i < n; ++i)
     {
-        // ImportanceSampleGGX
-        const float2 xi  = hammersley(i, n);
-        const float  phi = 2.0f * kPi * xi.x;
-        const float  ct  = std::sqrt(saturate((1.0f - xi.y) / (1.0f + (a2 - 1.0f) * xi.y)));
-        const float  st  = std::sqrt(saturate(1.0f - ct * ct));
-        const float3 H   = TX * (st * cos_(phi)) + TY * (st * sin_(phi)) + N * ct;
+        const float3 H   = ImportanceSampleGGX(hammersley(i, n), rough, N);
         const float3 L   = 2.0f * dot(V, H) * H - V;
         const float  NoL = clampf(dot(N, L), 0.0f, 1.0f), VoH = clampf(dot(V, H), 0.0f, 1.0f);
         if (!(NoL > 0.0f && VoH > 0.0f)) continue;

@@ -16,7 +16,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(_HERE, "_build", "liboracle_ibl.so")
 SOURCES = [os.path.join(_HERE, "oracle_ibl.cpp")]
-HEADERS = [os.path.join(_HERE, "oracle_math.h")]
+HEADERS = [os.path.join(_HERE, "oracle_math.h"), os.path.join(_HERE, "oracle_ibl_math.h")]
 # the flags of oracle/Makefile: scalar C++, no FMA contraction
 CXXFLAGS = ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fvisibility=hidden", "-pthread", "-shared"]
 

@@ -89,9 +89,11 @@ class Oracle:
     def set_frame_index(self, idx: int):
         self.L.orc_set_frame_index(self.h_, C.c_uint32(idx))
 
-    def brdf_lut(self, size: int = 512, num_samples: int = 512):
-        """Pre-integrated GGX table (PrecomputeBRDF.psh) into the plane "brdf_lut"; the reference uses 512 x 512, 512 samples."""
-        self.L.orc_brdf_lut(self.h_, int(size), C.c_uint32(num_samples))
+    def brdf_lut(self, size: int | tuple[int, int] = 512, num_samples: int = 512):
+        """Pre-integrated GGX table (PrecomputeBRDF.psh) into the plane "brdf_lut": `size` x `size`, or w x h for size = (w, h); the
+        reference uses 512 x 512, 512 samples."""
+        w, h = (size, size) if isinstance(size, int) else size
+        self.L.orc_brdf_lut(self.h_, int(w), int(h), C.c_uint32(num_samples))
 
     def set_reversed_depth(self, on: bool):
         """PostFXContext::FEATURE_FLAG_REVERSED_DEPTH (process-wide switch, like the reference's shader macro)."""

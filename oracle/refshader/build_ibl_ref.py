@@ -5,6 +5,8 @@ rewrites and harness protocol, read in place from the reference's tree) into a l
   ibl_irradiance__<type>_<opt>   ComputeIrradianceMap.psh with harness/irradiance_cube.inc
   ibl_prefilter__<type>_<opt>    PrefilterEnvMap.psh with harness/prefilter_env_map.inc
   with the macros PBR_Renderer::PrecomputeCubemaps sets (PBR_Renderer.cpp:794-798): ENV_MAP_TYPE (0 cube, 1 sphere), OPTIMIZE_SAMPLES.
+  brdf_lut__<n>                  PrecomputeBRDF.psh with harness/brdf_lut.inc and NUM_SAMPLES n (PBR_Renderer::PrecomputeBRDF uses 512),
+                                 built as build_ref.py builds a full-screen pass
 
 What the build supplies, in this library only:
   * the vertex and the pixel shader both declare cbConstants; each is flattened into a namespace of its own (ibvs, ibps), and the
@@ -13,7 +15,8 @@ What the build supplies, in this library only:
     shader is evaluated at the pixel centre; the `WORLD_POS` semantic is dropped like the SV_ ones;
   * `TextureCube<float4> g_EnvironmentMap` becomes `EnvCube<float4> g_EnvironmentMap`, the cube sampler of env_map_defs.inc with the
     seamless rule of DESIGN.md §2, as build_env_map_ref.py does for EnvMap.psh;
-  * ibl_defs.inc states the shaders' transcendentals as correctly rounded (DESIGN.md §2); hlsl.hpp is left as it is.
+  * ibl_defs.inc states the shaders' transcendentals and PrecomputeBRDF.psh's pow(x, 5.0) as correctly rounded (DESIGN.md §2); hlsl.hpp
+    is left as it is.
 
 Usage: python oracle/refshader/build_ibl_ref.py [--force]
 """
@@ -54,7 +57,23 @@ PASSES = [{"name": name(*k), "shader": "ComputeIrradianceMap.psh" if k[0] == "ir
            "macros": {"ENV_MAP_TYPE_CUBE": 0, "ENV_MAP_TYPE_SPHERE": 1, "ENV_MAP_TYPE": k[1], "OPTIMIZE_SAMPLES": k[2]}} for k in VARIANTS]
 
 
+BRDF_SAMPLES = (1, 2, 64, 512)
+
+
+def brdf_name(n: int) -> str:
+    return f"brdf_lut__{n}"
+
+
+BRDF_PASSES = [{"name": brdf_name(n), "shader": "PrecomputeBRDF.psh", "harness": "brdf_lut.inc", "macros": {"NUM_SAMPLES": f"{n}u"}, "brdf": True}
+               for n in BRDF_SAMPLES]
+
+
 def translation_unit(br, p: dict, idx: dict) -> str:
+    if p.get("brdf"):
+        core = open(os.path.join(HERE, "core_defs.inc")).read()
+        tu = br.translation_unit(p, idx)
+        assert tu.count(core) == 1
+        return tu.replace(core, core + open(os.path.join(HERE, "ibl_defs.inc")).read())
     ns = "refsh_ns_" + p["name"]
     drop = lambda t: re.sub(r":\s*(?:" + br.SEMANTICS + r"|WORLD_POS)\b", "", t)  # noqa: E731
     fst = br.flatten("FullScreenTriangleVSOutput.fxh", idx, set())  # what harness/common.inc's full-screen rasteriser is written against
@@ -108,7 +127,7 @@ def build(force: bool = False) -> str:
         return obj, ""
 
     with cf.ThreadPoolExecutor(max_workers=min(16, os.cpu_count() or 4)) as ex:
-        results = list(ex.map(compile_one, PASSES))
+        results = list(ex.map(compile_one, PASSES + BRDF_PASSES))
     errors = [e for _, e in results if e]
     if errors:
         raise RuntimeError("\n".join(errors))
@@ -140,6 +159,15 @@ def run(name_: str, levels, out, num_samples: int, face: int, roughness: float =
     r = fn(C.byref(a))
     if r != 0:
         raise RuntimeError(f"refsh_{name_} failed with {r} (1: wrong resource count, 2: wrong constant buffer)")
+
+
+def run_brdf(num_samples: int, out) -> None:
+    """PrecomputeBRDF.psh with NUM_SAMPLES `num_samples` (one of BRDF_SAMPLES) into `out` (h x w x 2 fp32), in place."""
+    global _lib
+    from oracle.refshader import refsh
+    if _lib is None:
+        _lib = C.CDLL(LIB)
+    refsh.run(brdf_name(num_samples), [], [out], library=_lib)
 
 
 if __name__ == "__main__":

@@ -83,10 +83,9 @@ PASSES = [
     _p("dof_postfilter", "DOF_ComputePostfilteredTexture.fx"),
     _p("dof_combine", "DOF_ComputeCombinedTexture.fx"),
 ] + [
-    # the compose step of the application (Hydrogent HnPostProcess.psh) and the table it samples (PBR PrecomputeBRDF.psh)
+    # the compose step of the application (Hydrogent HnPostProcess.psh); the table it samples (PBR PrecomputeBRDF.psh) is built with the
+    # IBL precomputation shaders by build_ibl_ref.py, under their statement of the transcendentals
     # HnPostProcessTask.cpp:219-225: VIEW_MODE = HN_VIEW_MODE_SHADED (0); the three debug modes only need to differ from it
     _p("compose_ibl", "HnPostProcess.psh", VIEW_MODE=0, VIEW_MODE_SCENE_DEPTH=101, VIEW_MODE_EDGE_MAP=102, VIEW_MODE_MESH_ID=103, TONE_MAPPING_MODE=0,
        CONVERT_OUTPUT_TO_SRGB=0),
-    _p("brdf_lut", "PrecomputeBRDF.psh", NUM_SAMPLES="512u"),
-    _p("brdf_lut__64", "PrecomputeBRDF.psh", NUM_SAMPLES="64u"),
 ]

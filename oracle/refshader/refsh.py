@@ -55,8 +55,9 @@ def _plane(a: np.ndarray) -> Plane:
     return Plane(a.ctypes.data, a.shape[1], a.shape[0], 1 if a.ndim == 2 else a.shape[2])
 
 
-def run(name: str, ins, outs, cbs=(), iparams=(), mask: np.ndarray | None = None, threads: int = 0) -> None:
-    """One full-screen pass of the reference shader `name`: `outs` (fp32 arrays, H x W [x C]) are written in place."""
+def run(name: str, ins, outs, cbs=(), iparams=(), mask: np.ndarray | None = None, threads: int = 0, library: C.CDLL | None = None) -> None:
+    """One full-screen pass of the reference shader `name`: `outs` (fp32 arrays, H x W [x C]) are written in place. `library`: another
+    library built with the same harness protocol (default librefshaders.so)."""
     ins = [np.ascontiguousarray(a) if a.dtype == np.uint32 else np.ascontiguousarray(a, np.float32) for a in ins]
     for o in outs:
         assert o.dtype == np.float32 and o.flags["C_CONTIGUOUS"]
@@ -71,7 +72,7 @@ def run(name: str, ins, outs, cbs=(), iparams=(), mask: np.ndarray | None = None
         assert m.shape == outs[0].shape[:2]
     a = Args(pin, len(ins), pout, len(outs), cb_ptr, cb_size, len(cbs), ip, len(iparams), m.ctypes.data if m is not None else None,
              threads or (os.cpu_count() or 1))
-    fn = getattr(lib(), "refsh_" + name)
+    fn = getattr(library or lib(), "refsh_" + name)
     fn.restype = C.c_int
     r = fn(C.byref(a))
     if r != 0:

@@ -2,7 +2,8 @@
 // default attribs into RGBA16_FLOAT textures of the default sizes, from Hydrogent's default dome (32 x 32 white, one level, a sphere
 // map; HnLight.cpp:667-685), then PrecomputeBRDF. Host-only translation unit: everything goes through the C++ header and the C-ABI.
 // Then the same with DFX_MAX_ENV_LEVELS levels on both sides: a white 4^2 cube with 16 levels into a 16-level prefiltered chain from 2^2.
-// Every irradiance and prefiltered texel of a white map is white; prints "ok" when they are and the BRDF table is finite.
+// Every irradiance and prefiltered texel of a white map is white; prints "ok" when they are and the BRDF table is finite. With a path
+// argument, PrecomputeBRDF's table (BRDF_LUT_Dim^2 texels, RG fp32, rows top to bottom) is written there.
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
@@ -30,7 +31,7 @@ static bool all_rgb_one(ITexture& t, float alpha)
     return true;
 }
 
-int main()
+int main(int argc, char** argv)
 {
     IDeviceContext ctx;
     ITexture       dome{32, 32, TEX_FORMAT_RGBA32_FLOAT};
@@ -66,6 +67,11 @@ int main()
     if (!renderer.GetPreintegratedGGX_SRV()->GetTexture()->ReadData(&ctx, lut.data())) return 5;
     for (float v : lut)
         if (!std::isfinite(v) || v < 0.0f || v > 1.5f) return std::printf("brdf %g\n", v), 6;
+    if (argc > 1)
+    {
+        std::FILE* f = std::fopen(argv[1], "wb");
+        if (!f || std::fwrite(lut.data(), sizeof(float), lut.size(), f) != lut.size() || std::fclose(f) != 0) return std::printf("cannot write %s\n", argv[1]), 10;
+    }
 
     // DFX_MAX_ENV_LEVELS levels: the source s_i = max(4 >> i, 1), the prefiltered chain s_m = max(2 >> m, 1)
     std::vector<std::unique_ptr<ITexture>>     src16;

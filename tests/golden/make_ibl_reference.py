@@ -10,7 +10,10 @@ Each case is a source map and a sample count; every case runs the 4^2 irradiance
   * sphere sources: 64 x 32 with 4 levels, 32 x 16 with one level, a sky with a sun 10^4 times brighter than the rest (64 x 32, 3
     levels), and Hydrogent's default dome (32 x 32 white, one level; HnLight.cpp:667-685);
   * sample counts 1, 2, 37 (not a power of two) and 64.
-Every output plane (the six faces of one level, fp32) is stored as the SHA-256 of its bytes.
+Beside them, PrecomputeBRDF.psh's pre-integrated GGX table (the same library, the same statement of the transcendentals) against
+oracle_compose_ibl.cpp's brdf_lut at 64 x 64 and 32 x 8 with 1, 2, 64 and 512 samples: power-of-two sizes, where the shader runner's
+interpolated texture coordinate is the oracle's (x + 0.5) / w exactly.
+Every output plane (the six faces of one level, fp32, or one table) is stored as the SHA-256 of its bytes.
 
     python tests/golden/make_ibl_reference.py
 """
@@ -29,6 +32,8 @@ import ibl_cases as IC  # noqa: E402
 OUT = os.path.join(HERE, "ibl_reference.npz")
 SIZE, LEVELS = 4, 3
 SAMPLES = (1, 2, 37, 64)
+BRDF_SIZES = ((64, 64), (32, 8))
+BRDF_SAMPLES = (1, 2, 64, 512)
 
 
 def sources() -> dict:
@@ -57,6 +62,23 @@ def planes(with_reference: bool):
                 for m in range(LEVELS):
                     s, r = max(SIZE >> m, 1), oi.roughness(m, LEVELS)
                     yield f"{key}/prefilter{m}", (ref("prefilter", t, o, lv, s, n, r) if with_reference else oi.prefilter(t, lv, s, r, n, bool(o)))
+    yield from brdf_tables(with_reference)
+
+
+def brdf_tables(with_reference: bool):
+    """Yields (key, (h, w, 2) fp32) for every BRDF table case: the reference shader or the oracle."""
+    from oracle import oracle_py as op
+    from oracle.refshader import build_ibl_ref as br
+    o = None if with_reference else op.Oracle(8, 8)
+    for w, h in BRDF_SIZES:
+        for n in BRDF_SAMPLES:
+            if with_reference:
+                lut = np.zeros((h, w, 2), np.float32)
+                br.run_brdf(n, lut)
+            else:
+                o.brdf_lut((w, h), n)
+                lut = o.get("brdf_lut")
+            yield f"brdf/{w}x{h}/n{n}", lut
 
 
 def run(with_reference: bool) -> dict:

@@ -236,12 +236,17 @@ def test_refusals(built):
 
 def test_cpp_pbr_renderer(built, tmp_path):
     """tests/cpp/ibl_driver.cpp drives include/dfx/PBR_Renderer.hpp: PrecomputeCubemaps with default attribs on a white sphere map (the
-    outputs are 1), the same with 16 source and 16 prefiltered levels, and PrecomputeBRDF."""
+    outputs are 1), the same with 16 source and 16 prefiltered levels, and PrecomputeBRDF, whose 512 x 512 table must be the oracle's
+    (512 samples) byte for byte."""
     exe = str(tmp_path / "ibl_driver")
     libdir = os.path.dirname(capi.LIB_PATH)
     r = subprocess.run(["g++", "-std=c++17", "-O1", "-Wall", "-Wextra", os.path.join(HERE, "cpp", "ibl_driver.cpp"), "-I", os.path.join(ROOT, "include"),
                         "-L", libdir, "-ldfx_b200", f"-Wl,-rpath,{libdir}", "-Wl,--allow-shlib-undefined", "-o", exe], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
-    r = subprocess.run([exe], capture_output=True, text=True)
+    table = str(tmp_path / "brdf_lut.bin")
+    r = subprocess.run([exe, table], capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "ok" in r.stdout
+    o = op.Oracle(8, 8)
+    o.brdf_lut(512, 512)
+    assert open(table, "rb").read() == o.get("brdf_lut").tobytes(), "PBR_Renderer::PrecomputeBRDF's table is not the oracle's"

@@ -2,8 +2,10 @@
 PrefilterEnvMap.psh, bit for bit (the bytes of every output level are compared through their SHA-256), in all eight variants of
 oracle/refshader/build_ibl_ref.py on the cases of tests/golden/make_ibl_reference.py: cube and sphere sources with one and several
 levels and the LOD clamp, a sun 10^4 times brighter than the rest, Hydrogent's white default dome, 1, 2, 37 and 64 samples,
-OPTIMIZE_SAMPLES 0 and 1, the irradiance cube and three prefiltered levels (roughness 0, 0.5, 1). The recorded shader outputs are
+OPTIMIZE_SAMPLES 0 and 1, the irradiance cube and three prefiltered levels (roughness 0, 0.5, 1); and PrecomputeBRDF.psh's GGX table
+against oracle_compose_ibl.cpp's at 64 x 64 and 32 x 8 with 1, 2, 64 and 512 samples. The recorded shader outputs are
 tests/golden/ibl_reference.npz; where the shader can be run, the fixture must be what it produces now."""
+import hashlib
 import importlib.util
 import os
 
@@ -24,9 +26,23 @@ def test_oracle_matches_committed_reference_outputs(built):
     m = _gen()
     want = np.load(m.OUT)
     got = m.run(with_reference=False)
-    assert set(got) == set(want.files) and len(got) == len(m.sources()) * len(m.SAMPLES) * 2 * (1 + m.LEVELS)
+    cubes = len(m.sources()) * len(m.SAMPLES) * 2 * (1 + m.LEVELS)
+    assert set(got) == set(want.files) and len(got) == cubes + len(m.BRDF_SIZES) * len(m.BRDF_SAMPLES)
     bad = [k for k in want.files if got[k].tobytes() != want[k].tobytes()]
     assert not bad, f"the oracle's IBL passes no longer reproduce the reference shaders on {len(bad)} planes:\n  " + "\n  ".join(bad[:20])
+
+
+def test_brdf_table_matches_the_reference_shader(built):
+    """PrecomputeBRDF.psh against oracle_compose_ibl.cpp's brdf_lut() under DESIGN.md §2's rule (one rounding per operation, cos / sin
+    correctly rounded, pow(x, 5) as ((x * x) * (x * x)) * x in double), bit for bit, at 64 x 64 and 32 x 8 with 1, 2, 64 and 512
+    samples: every table case of the committed reference outputs is present and reproduced."""
+    m = _gen()
+    want = np.load(m.OUT)
+    keys = [f"brdf/{w}x{h}/n{n}" for w, h in m.BRDF_SIZES for n in m.BRDF_SAMPLES]
+    assert set(keys) <= set(want.files)
+    got = {k: np.frombuffer(hashlib.sha256(np.ascontiguousarray(a).tobytes()).digest(), np.uint8) for k, a in m.brdf_tables(False)}
+    bad = [k for k in keys if got[k].tobytes() != want[k].tobytes()]
+    assert not bad, f"the oracle's BRDF table no longer reproduces PrecomputeBRDF.psh on {bad}"
 
 
 def test_cases_reach_the_lod_clamp_and_a_sun(built):

@@ -241,19 +241,6 @@ def test_oracle_refuses_a_bloom_pyramid_of_one_level(built):
         o.run("bloom")
 
 
-def test_brdf_table_bit_exact(shaders, case):
-    """PrecomputeBRDF.psh against oracle_compose_ibl.cpp's brdf_lut(), at two sample counts."""
-    from oracle import oracle_py as op
-    o = op.Oracle(W, H)
-    for size, samples, name in ((64, 512, "brdf_lut"), (32, 64, "brdf_lut__64")):     # powers of two, like the reference's 512 x 512 table
-        o.brdf_lut(size, samples)
-        want = o.get("brdf_lut")
-        got = np.zeros_like(want)
-        if shaders.live:
-            refsh.run(name, [], [got])
-        _check(shaders, case, {f"BRDF table {size} x {size}, {samples} samples": (got, want)})
-
-
 @pytest.mark.parametrize("size", [(128, 64), (157, 89)], ids=["128x64", "157x89"])
 def test_full_compose(shaders, case, size):
     """Hydrogent's HnPostProcess.psh (SSR re-weighted by the split-sum BRDF and exchanged for the specular IBL, then SSAO)
