@@ -18,6 +18,7 @@ HEADER_PATH = os.path.join(REPO_ROOT, "include", "dfx_b200.h")
 DFX_OK, DFX_ERR_INVALID_ARG, DFX_ERR_CUDA, DFX_ERR_NOT_PREPARED, DFX_ERR_UNSUPPORTED = range(5)
 FORMAT_R32F, FORMAT_RG32F, FORMAT_RGBA32F, FORMAT_R8U = 1, 2, 3, 4
 FORMAT_RGBA16F, FORMAT_RG16F, FORMAT_RG8U, FORMAT_RGBA8U = 5, 6, 7, 8   # transfer formats (unpack / pack only)
+FORMAT_R16U, FORMAT_RG16U = 9, 10   # D16_UNORM depth and RG16_UNORM (dfx_shadow_convert_to_filterable only)
 MAX_MIPS = 8
 
 TAA_FLAG_GAUSSIAN, TAA_FLAG_BICUBIC, TAA_FLAG_YCOCG = 1, 2, 4
@@ -153,6 +154,38 @@ ENV_MAP_OPTION_CONVERT_OUTPUT_TO_SRGB, ENV_MAP_OPTION_COMPUTE_MOTION_VECTORS, EN
 MAX_ENV_LEVELS = 16
 IRRADIANCE_CUBE_DIM, PREFILTERED_ENV_MAP_DIM = 64, 256
 DEFAULT_DIFFUSE_SAMPLES, DEFAULT_SPECULAR_SAMPLES = 8192, 256
+
+
+# BasicStructures.fxh SHADOW_MODE_* and MAX_CASCADES
+SHADOW_MODE_PCF, SHADOW_MODE_VSM, SHADOW_MODE_EVSM2, SHADOW_MODE_EVSM4 = 1, 2, 3, 4
+MAX_CASCADES = 8
+
+
+class CascadeAttribs(C.Structure):
+    """dfx_cascade_attribs == CascadeAttribs (BasicStructures.fxh:6-14, 64 bytes)."""
+    _fields_ = [("f4LightSpaceScale", C.c_float * 4), ("f4LightSpaceScaledBias", C.c_float * 4), ("f4StartEndZ", C.c_float * 4),
+                ("f4MarginProjSpace", C.c_float * 4)]
+
+
+class ShadowMapAttribs(C.Structure):
+    """dfx_shadow_map_attribs == ShadowMapAttribs (BasicStructures.fxh:28-67, the C++ form, 1200 bytes)."""
+    _fields_ = [("mWorldToLightView", Float4x4), ("Cascades", CascadeAttribs * MAX_CASCADES),
+                ("mWorldToShadowMapUVDepth", Float4x4 * MAX_CASCADES), ("fCascadeCamSpaceZEnd", C.c_float * MAX_CASCADES),
+                ("f4ShadowMapDim", C.c_float * 4),
+                ("iNumCascades", C.c_int32), ("fNumCascades", C.c_float), ("bVisualizeCascades", C.c_int32), ("bVisualizeShadowing", C.c_int32),
+                ("fReceiverPlaneDepthBiasClamp", C.c_float), ("fFixedDepthBias", C.c_float), ("fCascadeTransitionRegion", C.c_float),
+                ("iMaxAnisotropy", C.c_int32), ("fVSMBias", C.c_float), ("fVSMLightBleedingReduction", C.c_float),
+                ("fEVSMPositiveExponent", C.c_float), ("fEVSMNegativeExponent", C.c_float), ("bIs32BitEVSM", C.c_int32),
+                ("iFixedFilterSize", C.c_int32), ("fFilterWorldSize", C.c_float), ("fDummy", C.c_int32)]
+
+    @staticmethod
+    def default() -> "ShadowMapAttribs":
+        """The struct's DEFAULT_VALUEs; every field without one is zero."""
+        a = ShadowMapAttribs()
+        a.fReceiverPlaneDepthBiasClamp, a.fFixedDepthBias, a.fCascadeTransitionRegion, a.iMaxAnisotropy = 10.0, 1e-5, 0.1, 4
+        a.fVSMBias, a.fVSMLightBleedingReduction, a.fEVSMPositiveExponent, a.fEVSMNegativeExponent = 1e-4, 0.0, 40.0, 5.0
+        a.bIs32BitEVSM, a.iFixedFilterSize, a.fFilterWorldSize = 1, 3, 0.0
+        return a
 
 
 class BoundBoxAttribs(C.Structure):
@@ -301,6 +334,7 @@ class CoordinateGridRenderAttribs(C.Structure):
 
 assert C.sizeof(DOFAttribs) == 32 and C.sizeof(CoordinateGridAttribs) == 192 and C.sizeof(SelectionAttribs) == 48 and C.sizeof(EnvMapAttribs) == 80 and C.sizeof(BoundBoxAttribs) == 96
 assert C.sizeof(VectorFieldAttribs) == 56
+assert C.sizeof(CascadeAttribs) == 64 and C.sizeof(ShadowMapAttribs) == 1200
 
 
 class ChainConfigC(C.Structure):

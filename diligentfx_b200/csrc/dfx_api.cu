@@ -208,6 +208,8 @@ static size_t bytes_per_texel(int fmt)
         case DFX_FORMAT_RG16F: return 4;
         case DFX_FORMAT_RG8U: return 2;
         case DFX_FORMAT_RGBA8U: return 4;
+        case DFX_FORMAT_R16U: return 2;
+        case DFX_FORMAT_RG16U: return 4;
         default: return 0;
     }
 }
@@ -245,6 +247,7 @@ dfx_status dfx_plane_download(void* stream, const dfx_plane* src, void* host_dst
 dfx_status dfx_plane_fill(void* stream, const dfx_plane* dst, const float value[4])
 {
     DFX_REQUIRE(dst && dst->ptr && value, "null argument");
+    DFX_REQUIRE(dst->format != DFX_FORMAT_R16U && dst->format != DFX_FORMAT_RG16U, "dfx_plane_fill does not fill the UNORM16 shadow-map formats");
     if (dst->format == DFX_FORMAT_R8U)
     {
         DFX_CUDA(cudaMemset2DAsync(dst->ptr, dst->pitch_bytes, value[0] != 0.0f ? 1 : 0, dst->width, dst->height, as_stream(stream)));

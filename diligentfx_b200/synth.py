@@ -663,3 +663,32 @@ def motion_extreme(width: int, height: int, seed: int = 0) -> np.ndarray:
     pick = rng.random((height, width, 2)) < 0.3
     out[pick] = special[rng.integers(0, len(special), int(pick.sum()))]
     return out
+
+
+def shadow_cascades(n: int, width: int, height: int, seed: int = 0, d16: bool = False, hostile: bool = False) -> np.ndarray:
+    """Seeded depth of n shadow-map cascades as a light would render them: cleared to 1, then per cascade a few slanted ground and
+    wall planes and sphere occluders, nearer surfaces winning. d16: the D16_UNORM codes (uint16, round(saturate(z) * 65535)); otherwise
+    D32_FLOAT (float32). hostile (D32 only): a share of texels replaced by depth outside [0, 1], +-inf and NaN."""
+    rng = np.random.default_rng(seed)
+    y, x = np.meshgrid((np.arange(height) + 0.5) / height, (np.arange(width) + 0.5) / width, indexing="ij")
+    out = np.ones((n, height, width), np.float64)
+    for c in range(n):
+        z = out[c]
+        for _ in range(int(rng.integers(1, 4))):             # slanted planes: z = a + b x + c y, kept where inside [0, 1]
+            a, b, cc = rng.uniform(0.3, 0.9), rng.uniform(-0.4, 0.4), rng.uniform(-0.4, 0.4)
+            p = a + b * x + cc * y
+            z[:] = np.where((p >= 0) & (p < z), p, z)
+        for _ in range(int(rng.integers(2, 7))):             # spheres: the near cap of a ball of radius r at (cx, cy, cz)
+            cx, cy, r = rng.uniform(0, 1), rng.uniform(0, 1), rng.uniform(0.03, 0.3)
+            cz = rng.uniform(r, 1.0)
+            d2 = r * r - (x - cx) ** 2 - (y - cy) ** 2
+            s = cz - np.sqrt(np.maximum(d2, 0.0))
+            z[:] = np.where((d2 > 0) & (s < z), s, z)
+    if d16:
+        return np.rint(np.clip(out, 0.0, 1.0) * 65535.0).astype(np.uint16)
+    out = out.astype(np.float32)
+    if hostile:
+        special = np.array([np.nan, np.inf, -np.inf, -0.5, 1.5, -3.0, 7.0, -0.0, 3e38], np.float32)
+        pick = rng.random(out.shape) < 0.05
+        out[pick] = special[rng.integers(0, len(special), int(pick.sum()))]
+    return out

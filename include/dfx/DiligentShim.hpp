@@ -66,7 +66,10 @@ enum TEXTURE_FORMAT : Uint32
     TEX_FORMAT_RG16_FLOAT   = DFX_FORMAT_RG16F,
     TEX_FORMAT_RG8_UNORM    = DFX_FORMAT_RG8U,
     TEX_FORMAT_RGBA8_UNORM  = DFX_FORMAT_RGBA8U,
-    TEX_FORMAT_D32_FLOAT    = DFX_FORMAT_R32F // depth is an R32F plane here
+    TEX_FORMAT_D32_FLOAT    = DFX_FORMAT_R32F, // depth is an R32F plane here
+    // the shadow maps' own formats (ShadowMapManager.hpp)
+    TEX_FORMAT_D16_UNORM    = DFX_FORMAT_R16U,
+    TEX_FORMAT_RG16_UNORM   = DFX_FORMAT_RG16U
 };
 
 class IRenderDevice

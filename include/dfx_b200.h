@@ -61,7 +61,10 @@ typedef enum dfx_format
     DFX_FORMAT_RGBA16F = 5, /* scene colour, normal as the G-buffer stores them             8 B/texel */
     DFX_FORMAT_RG16F   = 6, /* motion vectors                                               4 B/texel */
     DFX_FORMAT_RG8U    = 7, /* material (roughness, metallic) UNORM                         2 B/texel */
-    DFX_FORMAT_RGBA8U  = 8  /* tone-mapped sRGB frame as a swap chain stores it             4 B/texel */
+    DFX_FORMAT_RGBA8U  = 8, /* tone-mapped sRGB frame as a swap chain stores it             4 B/texel */
+    /* shadow-map formats (dfx_shadow_convert_to_filterable only; every other entry refuses them) */
+    DFX_FORMAT_R16U    = 9, /* D16_UNORM depth: code k reads as k / 65535                  2 B/texel */
+    DFX_FORMAT_RG16U   = 10 /* RG16_UNORM variance shadow map: code k reads as k / 65535   4 B/texel */
 } dfx_format;
 
 /* A pitched 2-D array in HBM: row y starts at (char*)ptr + y*pitch_bytes. Stands in for ITextureView. */
@@ -746,6 +749,77 @@ DFX_API dfx_status dfx_pass_irradiance_cube(void* stream, int32_t env_type, cons
  * written by one launch. n_out = 1 is refused: the reference divides 0 by 0 there. */
 DFX_API dfx_status dfx_pass_prefilter_env_map(void* stream, int32_t env_type, const dfx_plane* env_levels, int32_t n_env,
                                               uint32_t num_samples, int32_t optimize_samples, const dfx_plane* out_levels, int32_t n_out);
+
+/* Shadow modes (BasicStructures.fxh SHADOW_MODE_*) and the most cascades a shadow map has (MAX_CASCADES). */
+#define DFX_SHADOW_MODE_PCF   1
+#define DFX_SHADOW_MODE_VSM   2
+#define DFX_SHADOW_MODE_EVSM2 3
+#define DFX_SHADOW_MODE_EVSM4 4
+#define DFX_MAX_CASCADES      8
+/* CascadeAttribs (BasicStructures.fxh:6-14), 64 bytes. */
+typedef struct dfx_cascade_attribs
+{
+    float f4LightSpaceScale[4];
+    float f4LightSpaceScaledBias[4];
+    float f4StartEndZ[4];
+    float f4MarginProjSpace[4]; /* the cascade margin in light projection space */
+} dfx_cascade_attribs;
+/* ShadowMapAttribs (BasicStructures.fxh:28-67, the C++ form), 1200 bytes; BOOL fields are 32-bit. The defaults are the struct's
+ * DEFAULT_VALUEs (capi.ShadowMapAttribs.default()). ConvertToFilterable reads iNumCascades, Cascades[i].f4LightSpaceScale.xy,
+ * fEVSMPositiveExponent, fEVSMNegativeExponent, bIs32BitEVSM, iFixedFilterSize and fFilterWorldSize. */
+typedef struct dfx_shadow_map_attribs
+{
+    dfx_float4x4        mWorldToLightView;
+    dfx_cascade_attribs Cascades[DFX_MAX_CASCADES];
+    dfx_float4x4        mWorldToShadowMapUVDepth[DFX_MAX_CASCADES];
+    float               fCascadeCamSpaceZEnd[DFX_MAX_CASCADES];
+    float               f4ShadowMapDim[4]; /* Width, Height, 1/Width, 1/Height */
+    int32_t iNumCascades;                  /* 0 */
+    float   fNumCascades;                  /* 0 */
+    int32_t bVisualizeCascades;            /* 0 */
+    int32_t bVisualizeShadowing;           /* 0 */
+    float   fReceiverPlaneDepthBiasClamp;  /* 10 */
+    float   fFixedDepthBias;               /* 1e-5 */
+    float   fCascadeTransitionRegion;      /* 0.1 */
+    int32_t iMaxAnisotropy;                /* 4 */
+    float   fVSMBias;                      /* 1e-4 */
+    float   fVSMLightBleedingReduction;    /* 0 */
+    float   fEVSMPositiveExponent;         /* 40 */
+    float   fEVSMNegativeExponent;         /* 5 */
+    int32_t bIs32BitEVSM;                  /* 1 */
+    int32_t iFixedFilterSize;              /* 3: a 3x3 filter */
+    float   fFilterWorldSize;              /* 0 */
+    int32_t fDummy;
+} dfx_shadow_map_attribs;
+/* The filter radii ConvertToFilterable uses for cascade `cascade` of a width x height shadow map (ShadowMapManager.cpp:560-579):
+ * (iFixedFilterSize - 1) / 2 on both axes when iFixedFilterSize > 0; otherwise, in float and in this order,
+ * fFilterWorldSize * f4LightSpaceScale.x * 0.5f / 2.f * width and the same with .y and height. Host only. Refuses a null pointer and
+ * a cascade outside 0..DFX_MAX_CASCADES-1. */
+DFX_API dfx_status dfx_shadow_filter_radii(const dfx_shadow_map_attribs* attribs, int32_t cascade, int32_t width, int32_t height,
+                                           float* horz_radius, float* vert_radius);
+/* ShadowMapManager::ConvertToFilterable (Components/src/ShadowMapManager.cpp:533-600; Shaders/Shadows/private/ShadowConversions.fx):
+ * the variance shadow maps of every cascade, from the depth the application rendered into each cascade. For cascade i, with the
+ * radii of dfx_shadow_filter_radii, VSMHorzPS (VSM) or EVSMHorzPS (EVSM2, EVSM4) then VertBlurPS, bit for bit by the rules of
+ * DESIGN.md §2: tap i of range = int(floor(r + 0.5)) weighs GetSampleWeight(i, r); moments are summed in tap order, one rounding per
+ * operation, then divided by the summed weight; an out-of-range depth tap reads 0 (warped for EVSM), an out-of-range row of the
+ * horizontal result reads 0; the horizontal result is stored in the filterable format (and read back from it) before the vertical
+ * pass; EVSM's exponents are clamped to 42 (32-bit) or 5.54 (16-bit) and exp is correctly rounded. iFixedFilterSize == 2 skips the
+ * vertical pass: the horizontal result is the filterable map.
+ *   shadow_map   n planes, one per cascade, all w x h (at most 16384 each way) and DFX_FORMAT_R16U (D16_UNORM) or R32F (D32_FLOAT).
+ *   filterable   n planes of the same size in the mode's filterable format, all the same: VSM RG16U or RG32F, EVSM2 RG16F or RG32F,
+ *                EVSM4 RGBA16F or RGBA32F; the 16-bit float stores round to nearest even, the UNORM store is
+ *                floor(saturate(v) * 65535 + 0.5) (NaN -> 0).
+ *   intermediate one w x h plane in the filterable format, the reference's one-slice intermediate. When every cascade's range is at
+ *                most 16 on both axes, one fused pass keeps the horizontal result on chip; the plane may then be NULL and is not
+ *                touched. Larger ranges run the reference's two passes per cascade through it.
+ * PCF returns DFX_OK and does nothing, as the reference does. Refuses an unknown mode, n outside 1..DFX_MAX_CASCADES,
+ * n != attribs->iNumCascades, bIs32BitEVSM disagreeing with the filterable format's width, formats or sizes other than these, a
+ * missing or mismatched intermediate where the two-pass path runs, a filterable slice (or the intermediate the two-pass path uses)
+ * whose bytes overlap another plane of the call (shadow-map slices may share memory: they are only read), and a radius that is negative or not finite
+ * or whose range is 2^15 or more. The work is enqueued on `stream` without host synchronisation. */
+DFX_API dfx_status dfx_shadow_convert_to_filterable(void* stream, int32_t mode, const dfx_shadow_map_attribs* attribs,
+                                                    const dfx_plane* shadow_map, int32_t n, const dfx_plane* filterable,
+                                                    const dfx_plane* intermediate);
 
 /* B the selected prim's bounding box (Components/src/BoundBoxRenderer.cpp:150-168 GetPSO, :257-277 Render; Shaders/Common/private/
  * BoundBox.vsh, BoundBox.psh:27-48 GetBoundBoxOutput), in place on the G-buffer's colour and motion planes. The 24 vertices of
