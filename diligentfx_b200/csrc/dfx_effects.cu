@@ -886,12 +886,34 @@ struct GraphPair
     cudaGraphExec_t front = nullptr, post = nullptr;
     int             kernels = 0; // kernel nodes of the two graphs: what one replay adds to dfx_launch_count()
 };
-void append_bytes(std::string& k, const void* p, size_t n) { k.append(static_cast<const char*>(p), n); }
+// the bytes of each of `v` onto the graph key `k`
+template <class... T> void append(std::string& k, const T&... v) { (k.append(reinterpret_cast<const char*>(&v), sizeof(v)), ...); }
 void append_plane(std::string& k, const dfx_plane* p)
 {
     static const dfx_plane none{};
-    append_bytes(k, p ? p : &none, sizeof(dfx_plane));
+    append(k, p ? *p : none);
 }
+
+// What the dfx_chain_set_* calls have switched on
+struct ChainFeatures
+{
+    uint32_t                    grid_flags = 0; // dfx_chain_set_coordinate_grid
+    dfx_coordinate_grid_attribs grid{};
+    bool                  sel_on = false; // dfx_chain_set_selection
+    dfx_selection_attribs sel{};
+    dfx_plane             sel_depth{};
+    int32_t               view_mode = DFX_VIEW_MODE_SHADED; // dfx_chain_set_view_mode
+    dfx_plane             mesh_id{};
+    float                 loading_factor = 0.0f;
+    float                 mv_elapsed = 0.0f; // dfx_chain_set_motion_vector_view (view_mode MOTION_VECTORS): the frame's ElapsedTime
+    bool                  env_on = false;    // dfx_chain_set_environment_map
+    int32_t               env_type = DFX_ENV_MAP_TYPE_CUBE;
+    dfx_pyramid           env_map{};
+    uint32_t              env_options = 0;
+    dfx_env_map_attribs   env{};
+    bool                  box_on = false; // dfx_chain_set_bound_box
+    dfx_bound_box_attribs box{};
+};
 } // namespace
 
 // HnPostProcessTask.cpp:625-654: every view mode but SHADED and WHITE_BASE_COLOR draws a renderer debug view, without SSR, SSAO,
@@ -900,10 +922,28 @@ static bool debug_view(int32_t m) { return m != DFX_VIEW_MODE_SHADED && m != DFX
 // the view modes HnPostProcess.psh itself draws (dfx_pass_compose_view)
 static bool compose_view_mode(int32_t m) { return m == DFX_VIEW_MODE_SCENE_DEPTH || m == DFX_VIEW_MODE_EDGE_MAP || m == DFX_VIEW_MODE_MESH_ID; }
 
+// The stages the switched-on features are drawn in: dfx_chain_create, dfx_chain_set_config and every setter refuse what this refuses.
+// E and B draw into the G-buffer and need no stage; with disable_taa the final compose draws the selection and the debug views.
+static dfx_status check_stages(const ChainFeatures& ft, const dfx_chain_config& cfg)
+{
+    const bool taa = !cfg.disable_taa, mv = ft.view_mode == DFX_VIEW_MODE_MOTION_VECTORS;
+    const struct { bool on; uint32_t need; const char *what, *stages; } rules[] = {
+        {!taa, DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP, "disable_taa draws the frame in the final compose", "DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TONEMAP"},
+        {ft.grid_flags != 0, DFX_CHAIN_STAGE_TONEMAP, "the coordinate grid is drawn in the tone-map step", "DFX_CHAIN_STAGE_TONEMAP"},
+        {mv, DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP, "the motion-vector view is drawn by the final compose", "DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TONEMAP"},
+        {taa && ft.sel_on, DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TAA, "the selection outline is drawn on the composed colour before TAA", "DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TAA"},
+        {taa && debug_view(ft.view_mode) && !mv, DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TAA, "a debug view mode is drawn by the compose before TAA", "DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TAA"},
+    };
+    for (const auto& r : rules)
+        if (r.on && (cfg.stages & r.need) != r.need) return set_error(DFX_ERR_INVALID_ARG, "%s: the stage mask must include %s", r.what, r.stages);
+    return DFX_OK;
+}
+
 static_assert(sizeof(dfx_chain_config) == 284, "dfx_chain_config layout (mirrored by diligentfx_b200/capi.py ChainConfigC)");
 struct dfx_chain
 {
     dfx_chain_config cfg{};
+    ChainFeatures    ft;
     int              w = 0, h = 0;
     dfx_postfx*      pfx   = nullptr;
     dfx_ssao*        ssao  = nullptr;
@@ -918,25 +958,9 @@ struct dfx_chain
     uint32_t         last_frame = ~0u;
     bool             graphs_ok  = true;
     std::map<std::string, GraphPair> graphs;
-    uint32_t                    grid_flags = 0; // dfx_chain_set_coordinate_grid
-    dfx_coordinate_grid_attribs grid{};
-    bool                  sel_on = false; // dfx_chain_set_selection
-    dfx_selection_attribs sel{};
-    dfx_plane             sel_depth{};
-    bool                  sel_taa_reset = false; // the selection changed: the next frame resets TAA's history
-    PlaneOwner            sel_loc, sel_scratch;
-    int32_t               view_mode = DFX_VIEW_MODE_SHADED; // dfx_chain_set_view_mode
-    dfx_plane             mesh_id{};
-    float                 loading_factor = 0.0f;
-    bool                  env_on = false; // dfx_chain_set_environment_map
-    int32_t               env_type = DFX_ENV_MAP_TYPE_CUBE;
-    dfx_pyramid           env_map{};
-    uint32_t              env_options = 0;
-    dfx_env_map_attribs   env{};
-    bool                  box_on = false; // dfx_chain_set_bound_box
-    dfx_bound_box_attribs box{};
-    float                 mv_elapsed = 0.0f; // dfx_chain_set_motion_vector_view (view_mode MOTION_VECTORS): the frame's ElapsedTime
-    PlaneOwner            mv_owner;          // the vector field's owner plane, all zero between frames
+    bool             sel_taa_reset = false; // the selection changed: the next frame resets TAA's history
+    PlaneOwner       sel_loc, sel_scratch;
+    PlaneOwner       mv_owner; // the vector field's owner plane, all zero between frames
     dfx_chain_stats  stats{};
 
     void drop_graphs()
@@ -947,6 +971,13 @@ struct dfx_chain
             if (g.second.post) cudaGraphExecDestroy(g.second.post);
         }
         graphs.clear();
+    }
+    // a setter's last step: `next` replaces the features if the stage mask draws them
+    dfx_status commit(const ChainFeatures& next)
+    {
+        const dfx_status st = check_stages(next, cfg);
+        if (st == DFX_OK) ft = next;
+        return st;
     }
     ~dfx_chain()
     {
@@ -979,19 +1010,14 @@ extern "C" void dfx_chain_config_default(dfx_chain_config* c)
 extern "C" dfx_status dfx_chain_create(int32_t width, int32_t height, const dfx_chain_config* config, dfx_chain** out)
 {
     DFX_REQUIRE(out && width > 0 && height > 0, "bad arguments");
+    dfx_chain_config cfg;
+    dfx_chain_config_default(&cfg);
+    if (config) cfg = *config;
+    dfx_status st = check_stages(ChainFeatures{}, cfg);
+    if (st != DFX_OK) return st;
     dfx_chain* c = new (std::nothrow) dfx_chain;
     DFX_REQUIRE(c, "out of memory");
-    c->w = width, c->h = height;
-    if (config)
-        c->cfg = *config;
-    else
-        dfx_chain_config_default(&c->cfg);
-    if (c->cfg.disable_taa && (~c->cfg.stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP)))
-    {
-        delete c;
-        return set_error(DFX_ERR_INVALID_ARG, "disable_taa draws the frame in the final compose: the stage mask must include DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TONEMAP");
-    }
-    dfx_status st = DFX_OK;
+    c->w = width, c->h = height, c->cfg = cfg;
     if (st == DFX_OK) st = dfx_postfx_create(&c->pfx);
     if (st == DFX_OK) st = dfx_ssao_create(&c->ssao);
     if (st == DFX_OK) st = dfx_ssr_create(&c->ssr);
@@ -1017,23 +1043,14 @@ extern "C" void dfx_chain_destroy(dfx_chain* c) { delete c; }
 extern "C" dfx_status dfx_chain_set_config(dfx_chain* c, const dfx_chain_config* config)
 {
     DFX_REQUIRE(c && config, "null argument");
+    const dfx_status st = check_stages(c->ft, *config);
+    if (st != DFX_OK) return st;
     // The graph cache is keyed by the configuration bytes, so a change of attribute values just stops hitting the old entries. A
     // change of feature flags or stages, however, makes the effects re-create their planes: every recorded graph then points at
     // freed memory and must go.
     const dfx_chain_config& o = c->cfg;
     const bool realloc = o.postfx_flags != config->postfx_flags || o.ssao_flags != config->ssao_flags || o.ssr_flags != config->ssr_flags || o.taa_flags != config->taa_flags ||
                          o.dof_flags != config->dof_flags || o.enable_dof != config->enable_dof || o.stages != config->stages || o.fuse != config->fuse;
-    if (c->grid_flags && !(config->stages & DFX_CHAIN_STAGE_TONEMAP))
-        return set_error(DFX_ERR_INVALID_ARG, "the coordinate grid is drawn in the tone-map step: a stage mask without DFX_CHAIN_STAGE_TONEMAP is refused while it is on");
-    if (config->disable_taa && (~config->stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP)))
-        return set_error(DFX_ERR_INVALID_ARG, "disable_taa draws the frame in the final compose: the stage mask must include DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TONEMAP");
-    if (c->sel_on && !config->disable_taa && (~config->stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TAA)))
-        return set_error(DFX_ERR_INVALID_ARG, "the selection outline is drawn on the composed colour before TAA: a stage mask without DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TAA is refused while it is on");
-    if (c->view_mode == DFX_VIEW_MODE_MOTION_VECTORS && (~config->stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP)))
-        return set_error(DFX_ERR_INVALID_ARG, "the motion-vector view is drawn by the final compose: a stage mask without DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TONEMAP is refused while it is on");
-    if (debug_view(c->view_mode) && c->view_mode != DFX_VIEW_MODE_MOTION_VECTORS && !config->disable_taa &&
-        (~config->stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TAA)))
-        return set_error(DFX_ERR_INVALID_ARG, "a debug view mode is drawn by the compose before TAA: a stage mask without DFX_CHAIN_STAGE_COMPOSE and DFX_CHAIN_STAGE_TAA is refused while it is on");
     if (realloc || c->graphs.size() > 16)
     {
         DFX_CUDA(cudaDeviceSynchronize()); // a graph that is still executing must not be destroyed
@@ -1046,35 +1063,31 @@ extern "C" dfx_status dfx_chain_set_coordinate_grid(dfx_chain* c, uint32_t flags
 {
     DFX_REQUIRE(c, "null argument");
     if (flags & ~DFX_GRID_FEATURE_FLAG_ALL) return set_error(DFX_ERR_UNSUPPORTED, "unknown coordinate grid feature flags 0x%x", flags);
-    DFX_REQUIRE(!flags || (c->cfg.stages & DFX_CHAIN_STAGE_TONEMAP), "the coordinate grid is drawn in the tone-map step: the chain's stage mask has no DFX_CHAIN_STAGE_TONEMAP");
-    c->grid_flags = flags;
-    if (attribs)
-        c->grid = *attribs;
-    else
-        dfx_coordinate_grid_attribs_default(&c->grid);
-    return DFX_OK; // graphs are keyed on (flags, attribs): the next frame records or replays the matching one
+    ChainFeatures next = c->ft;
+    next.grid_flags    = flags;
+    dfx_coordinate_grid_attribs_default(&next.grid);
+    if (attribs) next.grid = *attribs;
+    return c->commit(next);
 }
 extern "C" dfx_status dfx_chain_set_selection(dfx_chain* c, const dfx_selection_attribs* attribs, const dfx_plane* selection_depth)
 {
     DFX_REQUIRE(c, "null argument");
     if (attribs)
     {
-        // with disable_taa, disable_taa's own requirement (COMPOSE + TONEMAP) already holds
-        DFX_REQUIRE(c->cfg.disable_taa || ((c->cfg.stages & DFX_CHAIN_STAGE_COMPOSE) && (c->cfg.stages & DFX_CHAIN_STAGE_TAA)),
-                    "the selection outline is drawn on the composed colour before TAA: the chain's stage mask lacks DFX_CHAIN_STAGE_COMPOSE or DFX_CHAIN_STAGE_TAA");
         DFX_REQUIRE(std::isfinite(attribs->SelectionOutlineWidth) && attribs->SelectionOutlineWidth > 0.0f, "SelectionOutlineWidth must be positive and finite");
         View<const float> v;
         DFX_REQUIRE(make_view<const float>(selection_depth, DFX_FORMAT_R32F, v), "bad plane 'selection_depth' (null, wrong format, pitch or alignment)");
         DFX_REQUIRE(v.w == c->w && v.h == c->h, "the selection depth plane is %dx%d, the chain %dx%d", v.w, v.h, c->w, c->h);
     }
+    ChainFeatures next = c->ft;
+    next.sel_on        = attribs != nullptr;
+    next.sel           = attribs ? *attribs : dfx_selection_attribs{};
+    next.sel_depth     = attribs ? *selection_depth : dfx_plane{};
     // HnProcessSelectionTask.cpp:293-301: a different selected prim (none while off) resets TAA
-    const bool     on = attribs != nullptr;
-    const uint32_t id = on ? attribs->selection_id : 0u;
-    if (on != c->sel_on || (on && id != c->sel.selection_id)) c->sel_taa_reset = true;
-    c->sel_on = on;
-    if (on) c->sel = *attribs, c->sel_depth = *selection_depth;
-    else c->sel = dfx_selection_attribs{}, c->sel_depth = dfx_plane{};
-    return DFX_OK; // graphs are keyed on (attribs, plane): the next frame records or replays the matching one
+    const bool reset   = next.sel_on != c->ft.sel_on || (next.sel_on && next.sel.selection_id != c->ft.sel.selection_id);
+    const dfx_status st = c->commit(next);
+    if (st == DFX_OK && reset) c->sel_taa_reset = true;
+    return st;
 }
 extern "C" dfx_status dfx_chain_set_view_mode(dfx_chain* c, int32_t view_mode, const dfx_plane* mesh_id, float loading_animation_factor)
 {
@@ -1082,30 +1095,26 @@ extern "C" dfx_status dfx_chain_set_view_mode(dfx_chain* c, int32_t view_mode, c
     if (view_mode < 0 || view_mode >= DFX_VIEW_MODE_COUNT) return set_error(DFX_ERR_INVALID_ARG, "unknown view mode %d", view_mode);
     if (view_mode == DFX_VIEW_MODE_MOTION_VECTORS)
         return set_error(DFX_ERR_UNSUPPORTED, "the motion-vector view takes the frame's elapsed time: use dfx_chain_set_motion_vector_view");
-    if (debug_view(view_mode))
-    {
-        const uint32_t need = c->cfg.disable_taa ? DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP : DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TAA;
-        DFX_REQUIRE(!(~c->cfg.stages & need), "a debug view mode is drawn by the compose: the chain's stage mask lacks DFX_CHAIN_STAGE_COMPOSE or %s",
-                    c->cfg.disable_taa ? "DFX_CHAIN_STAGE_TONEMAP" : "DFX_CHAIN_STAGE_TAA");
-    }
     if (view_mode == DFX_VIEW_MODE_MESH_ID)
     {
         View<const float> v;
         DFX_REQUIRE(make_view<const float>(mesh_id, DFX_FORMAT_R32F, v), "bad plane 'mesh_id' (R32F; null, wrong format, pitch or alignment)");
         DFX_REQUIRE(v.w == c->w && v.h == c->h, "the mesh ID plane is %dx%d, the chain %dx%d", v.w, v.h, c->w, c->h);
     }
-    c->view_mode      = view_mode;
-    c->mesh_id        = view_mode == DFX_VIEW_MODE_MESH_ID ? *mesh_id : dfx_plane{};
-    c->loading_factor = loading_animation_factor;
-    return DFX_OK; // graphs are keyed on (view mode, plane, factor): the next frame records or replays the matching one
+    ChainFeatures next  = c->ft;
+    next.view_mode      = view_mode;
+    next.mesh_id        = view_mode == DFX_VIEW_MODE_MESH_ID ? *mesh_id : dfx_plane{};
+    next.loading_factor = loading_animation_factor;
+    return c->commit(next);
 }
 extern "C" dfx_status dfx_chain_set_environment_map(dfx_chain* c, int32_t type, const dfx_pyramid* env_map, uint32_t options, const dfx_env_map_attribs* attribs)
 {
     DFX_REQUIRE(c, "null argument");
+    ChainFeatures next = c->ft;
     if (!env_map)
     {
-        c->env_on = false, c->env_map = dfx_pyramid{};
-        return DFX_OK;
+        next.env_on = false, next.env_map = dfx_pyramid{};
+        return c->commit(next);
     }
     // HnRenderEnvMapTask.cpp:162-216: tone mapping is left to the post-process task; the dome light's colour * intensity is the scale
     dfx_env_map_attribs a;
@@ -1121,37 +1130,29 @@ extern "C" dfx_status dfx_chain_set_environment_map(dfx_chain* c, int32_t type, 
                 "the chain sets motion vectors (always on) and reverse depth (from the reversed-depth flag) itself: pass DFX_ENV_MAP_OPTION_CONVERT_OUTPUT_TO_SRGB or 0");
     const dfx_status st = env_map_check(type, env_map, options, &a);
     if (st != DFX_OK) return st;
-    c->env_on = true, c->env_type = type, c->env_map = *env_map, c->env_options = options, c->env = a;
-    return DFX_OK; // graphs are keyed on (type, map, options, attribs): the next frame records or replays the matching one
+    next.env_on = true, next.env_type = type, next.env_map = *env_map, next.env_options = options, next.env = a;
+    return c->commit(next);
 }
 extern "C" dfx_status dfx_chain_set_bound_box(dfx_chain* c, const dfx_bound_box_attribs* attribs)
 {
     DFX_REQUIRE(c, "null argument");
-    if (!attribs)
-    {
-        c->box_on = false;
-        return DFX_OK;
-    }
-    const dfx_status st = bound_box_check(attribs);
+    const dfx_status st = attribs ? bound_box_check(attribs) : DFX_OK;
     if (st != DFX_OK) return st;
-    c->box_on = true, c->box = *attribs;
-    c->box.Color[3] = 0.0f; // HnRenderBoundBoxTask's PS main: float4(Color.rgb, 0.0) (HnRenderBoundBoxTask.cpp:90)
-    return DFX_OK;          // graphs are keyed on the attribs: the next frame records or replays the matching one
+    ChainFeatures next = c->ft;
+    next.box_on        = attribs != nullptr;
+    if (attribs) next.box = *attribs, next.box.Color[3] = 0.0f; // HnRenderBoundBoxTask's PS main: float4(Color.rgb, 0.0) (HnRenderBoundBoxTask.cpp:90)
+    return c->commit(next);
 }
 extern "C" dfx_status dfx_chain_set_motion_vector_view(dfx_chain* c, int32_t on, float elapsed_time)
 {
     DFX_REQUIRE(c, "null argument");
-    if (!on)
-    {
-        if (c->view_mode == DFX_VIEW_MODE_MOTION_VECTORS) c->view_mode = DFX_VIEW_MODE_SHADED;
-        return DFX_OK;
-    }
-    DFX_REQUIRE(std::isfinite(elapsed_time), "elapsed_time must be finite");
-    DFX_REQUIRE(!(~c->cfg.stages & (DFX_CHAIN_STAGE_COMPOSE | DFX_CHAIN_STAGE_TONEMAP)),
-                "the motion-vector view is drawn by the final compose: the chain's stage mask lacks DFX_CHAIN_STAGE_COMPOSE or DFX_CHAIN_STAGE_TONEMAP");
-    c->view_mode = DFX_VIEW_MODE_MOTION_VECTORS, c->mesh_id = dfx_plane{}, c->loading_factor = 0.0f;
-    c->mv_elapsed = elapsed_time;
-    return DFX_OK; // graphs are keyed on the mode only: the elapsed time reaches the field's launches, which run after the graph
+    DFX_REQUIRE(!on || std::isfinite(elapsed_time), "elapsed_time must be finite");
+    ChainFeatures next = c->ft;
+    if (on)
+        next.view_mode = DFX_VIEW_MODE_MOTION_VECTORS, next.mesh_id = dfx_plane{}, next.loading_factor = 0.0f, next.mv_elapsed = elapsed_time;
+    else if (next.view_mode == DFX_VIEW_MODE_MOTION_VECTORS)
+        next.view_mode = DFX_VIEW_MODE_SHADED;
+    return c->commit(next);
 }
 extern "C" dfx_status dfx_chain_get_config(const dfx_chain* c, dfx_chain_config* out)
 {
@@ -1192,26 +1193,73 @@ extern "C" dfx_status dfx_chain_join(dfx_chain* c, void* stream)
 
 namespace
 {
+// What one frame runs, decided by plan_frame: record_front / record_post, the graph key and the replay test read it
 struct FrameCtx
 {
-    dfx_chain*             c;
-    const dfx_chain_frame* f;
-    uint32_t               st;
-    bool                   side_ao, side_post, fuse_compose, fuse_tonemap, with_dof, grid;
-    bool                   final_compose;        // disable_taa: F writes the frame, nothing runs after it
-    bool                   sel, taa_reset;       // selection on; TAA resets its history this frame
-    dfx_selection_attribs  sel_shader;           // the selection attribs with the outline colours as O sees them
-    bool                   front;                // PostFX prepare, S1, S2 and A2 run as one pass (dfx_pass_front_prepare) before the fork
-    bool                   debug;                // a renderer debug view: no SSR, SSAO, Bloom or DoF
-    bool                   env;                  // E draws the environment map into the frame's colour and motion first
-    bool                   box;                  // B draws the bounding box into them next
-    bool                   mv;                   // the motion-vector view: F, then the vector field over ldr_out
+    const dfx_chain*       c = nullptr;
+    const dfx_chain_frame* f = nullptr;
+    uint32_t               st = 0; // the stages that run
+    // a renderer debug view; the motion-vector view; F or V writes the frame and nothing runs after it (disable_taa or the motion-vector view)
+    bool debug = false, mv = false, final_compose = false;
+    bool with_dof = false, side_ao = false, side_post = false, fuse_compose = false, fuse_tonemap = false, grid = false;
+    bool env = false, box = false; // E, then B, draw into the frame's colour and motion first, with these options
+    uint32_t env_options = 0, box_options = 0;
+    bool sel = false, taa_reset = false; // selection on; TAA resets its history this frame
+    dfx_selection_attribs sel_shader{};  // the selection attribs with the outline colours as O sees them
+    bool upload_cameras = false;         // a kernel of this frame reads the cameras or the frame index
+    bool front = false;                  // PostFX prepare, S1, S2 and A2 run as one pass (dfx_pass_front_prepare) before the fork
 };
+
+FrameCtx plan_frame(const dfx_chain& c, const dfx_chain_frame& f)
+{
+    const dfx_chain_config& cfg = c.cfg;
+    const ChainFeatures&    ft  = c.ft;
+    FrameCtx                x;
+    x.c = &c, x.f = &f;
+    // With TAA off there is no TAA, hence no Bloom and no DepthOfField (HnPostProcessTask.cpp:652-654). A debug view mode runs no SSR,
+    // SSAO, Bloom or DepthOfField (:625-654), and PostFX only where TAA runs (:788)
+    x.debug = debug_view(ft.view_mode);
+    // The motion-vector view switches TAA off (:652) and with it PostFX (:788): F draws the frame, the vector field goes over it
+    x.mv            = ft.view_mode == DFX_VIEW_MODE_MOTION_VECTORS;
+    x.final_compose = cfg.disable_taa != 0 || x.mv;
+    x.st            = x.final_compose ? cfg.stages & ~(DFX_CHAIN_STAGE_TAA | DFX_CHAIN_STAGE_BLOOM) : cfg.stages;
+    if (x.debug) x.st &= ~(DFX_CHAIN_STAGE_SSR | DFX_CHAIN_STAGE_SSAO | DFX_CHAIN_STAGE_BLOOM | (x.final_compose ? DFX_CHAIN_STAGE_POSTFX : 0u));
+    // With the grid on, its step reads the caller's depth plane and the camera of this frame: Bloom + the grid step stay on the
+    // caller's stream, in order with what the caller does to its planes next, and the Bloom composite runs unfused before it.
+    x.grid      = ft.grid_flags != 0;
+    x.with_dof  = cfg.enable_dof != 0 && !x.final_compose && !x.debug;
+    x.side_ao   = cfg.overlap && (x.st & DFX_CHAIN_STAGE_SSAO) && (x.st & DFX_CHAIN_STAGE_SSR);
+    x.side_post = cfg.overlap && (x.st & DFX_CHAIN_STAGE_BLOOM) && (x.st & DFX_CHAIN_STAGE_TAA) && !x.with_dof && !x.grid;
+    // With selection on, O runs between the compose and TAA: the compose runs unfused
+    x.sel          = ft.sel_on;
+    x.taa_reset    = c.sel_taa_reset;
+    x.fuse_compose = cfg.fuse && (x.st & DFX_CHAIN_STAGE_COMPOSE) && (x.st & DFX_CHAIN_STAGE_TAA) && !x.sel && !compose_view_mode(ft.view_mode);
+    x.fuse_tonemap = cfg.fuse && (x.st & DFX_CHAIN_STAGE_BLOOM) && (x.st & DFX_CHAIN_STAGE_TONEMAP) && (c.w % 2 == 0) && (c.h % 2 == 0) && !x.grid;
+    // HnPostProcessTask.cpp:840-850: with TAA on and a tone map after it, the outline colours are reverse-tone-mapped
+    x.sel_shader = ft.sel;
+    if (x.sel && !x.final_compose && cfg.tonemap.iToneMappingMode != DFX_TONE_MAPPING_MODE_NONE)
+    {
+        dfx_reverse_exp_tone_map(ft.sel.SelectionColor, cfg.tonemap.fMiddleGray, cfg.ave_log_lum, x.sel_shader.SelectionColor);
+        dfx_reverse_exp_tone_map(ft.sel.OccludedSelectionColor, cfg.tonemap.fMiddleGray, cfg.ave_log_lum, x.sel_shader.OccludedSelectionColor);
+    }
+    const bool reversed = (cfg.postfx_flags & DFX_POSTFX_FEATURE_FLAG_REVERSED_DEPTH) != 0;
+    x.env         = ft.env_on && ft.view_mode != DFX_VIEW_MODE_SCENE_DEPTH; // HnRenderEnvMapTask::IsActive (HnRenderEnvMapTask.cpp:85-94)
+    x.env_options = ft.env_options | DFX_ENV_MAP_OPTION_COMPUTE_MOTION_VECTORS | (reversed ? DFX_ENV_MAP_OPTION_USE_REVERSE_DEPTH : 0u);
+    x.box         = ft.box_on; // HnRenderBoundBoxTask has no IsActive: every view mode
+    x.box_options = DFX_BOUND_BOX_OPTION_COMPUTE_MOTION_VECTORS | (reversed ? DFX_BOUND_BOX_OPTION_USE_REVERSE_DEPTH : 0u);
+    x.upload_cameras = (x.st & DFX_CHAIN_STAGE_POSTFX) || x.grid || x.env || x.box || compose_view_mode(ft.view_mode);
+    // the front pass needs every pass it replaces in this frame, at full resolution; dfx_tune "front_fused" = 0 keeps the separate
+    // passes. Whether the pyramids are deep enough for it is known once SSR and SSAO are prepared (dfx_chain_execute).
+    const uint32_t front_stages = DFX_CHAIN_STAGE_POSTFX | DFX_CHAIN_STAGE_SSR | DFX_CHAIN_STAGE_SSAO;
+    x.front = cfg.fuse && (x.st & front_stages) == front_stages && !(cfg.ssr_flags & DFX_SSR_FEATURE_FLAG_HALF_RESOLUTION) &&
+              !(cfg.ssao_flags & DFX_SSAO_FEATURE_FLAG_HALF_RESOLUTION) && dfx_tune_get("front_fused", 1);
+    return x;
+}
 
 // P0, then P1-P3 + S1 + S2 + A2 in one pass on `s`; SSR and SSAO Execute then skip S1 / S2 and A2
 dfx_status front_launch(const FrameCtx& x, cudaStream_t s)
 {
-    dfx_chain*              c   = x.c;
+    const dfx_chain*        c   = x.c;
     const dfx_chain_frame*  f   = x.f;
     const dfx_chain_config& cfg = c->cfg;
     dfx_postfx*             pfx = c->pfx;
@@ -1235,25 +1283,16 @@ dfx_status front_launch(const FrameCtx& x, cudaStream_t s)
 // PostFX .. TAA [.. DoF] on `s` (the SSAO passes fork to the chain's second stream and join before the compose). `*color_out` = what Bloom reads.
 dfx_status record_front(const FrameCtx& x, cudaStream_t s, dfx_plane* color_out)
 {
-    dfx_chain*             c   = x.c;
-    const dfx_chain_frame* f   = x.f;
+    const dfx_chain*        c   = x.c;
+    const ChainFeatures&    ft  = c->ft;
+    const dfx_chain_frame*  f   = x.f;
     const dfx_chain_config& cfg = c->cfg;
-    dfx_status             st;
+    dfx_status              st;
     // E (HnRenderEnvMapTask, before the post-process task): the sky and its motion into the frame's G-buffer, in place
-    if (x.env)
-    {
-        const uint32_t opts = c->env_options | DFX_ENV_MAP_OPTION_COMPUTE_MOTION_VECTORS |
-                              ((cfg.postfx_flags & DFX_POSTFX_FEATURE_FLAG_REVERSED_DEPTH) ? DFX_ENV_MAP_OPTION_USE_REVERSE_DEPTH : 0u);
-        if ((st = dfx_pass_env_map(s, c->pfx->cams_dev, c->env_type, &c->env_map, opts, &c->env, f->depth, f->color, f->motion, dfx_rows{0, c->h})) != DFX_OK)
-            return st;
-    }
+    if (x.env && (st = dfx_pass_env_map(s, c->pfx->cams_dev, ft.env_type, &ft.env_map, x.env_options, &ft.env, f->depth, f->color, f->motion, dfx_rows{0, c->h})) != DFX_OK)
+        return st;
     // B (HnRenderBoundBoxTask, right after E in the same render pass): the box's colour and its own motion, in place
-    if (x.box)
-    {
-        const uint32_t opts = DFX_BOUND_BOX_OPTION_COMPUTE_MOTION_VECTORS |
-                              ((cfg.postfx_flags & DFX_POSTFX_FEATURE_FLAG_REVERSED_DEPTH) ? DFX_BOUND_BOX_OPTION_USE_REVERSE_DEPTH : 0u);
-        if ((st = dfx_pass_bound_box(s, c->pfx->cams_dev, &c->box, opts, f->depth, f->color, f->motion, dfx_rows{0, c->h})) != DFX_OK) return st;
-    }
+    if (x.box && (st = dfx_pass_bound_box(s, c->pfx->cams_dev, &ft.box, x.box_options, f->depth, f->color, f->motion, dfx_rows{0, c->h})) != DFX_OK) return st;
     if (x.front)
     {
         if ((st = front_launch(x, s)) != DFX_OK) return st;
@@ -1276,7 +1315,7 @@ dfx_status record_front(const FrameCtx& x, cudaStream_t s, dfx_plane* color_out)
         if ((st = dfx_ssao_execute(c->ssao, &a)) != DFX_OK) return st;
     }
     // J depends on the selection plane only: it runs beside SSR with the SSAO passes
-    if (x.sel && (st = dfx_pass_closest_selected_location(x.side_ao ? c->ao_stream : s, c->sel.ClearDepth, c->sel.SelectionOutlineWidth, &c->sel_depth,
+    if (x.sel && (st = dfx_pass_closest_selected_location(x.side_ao ? c->ao_stream : s, ft.sel.ClearDepth, ft.sel.SelectionOutlineWidth, &ft.sel_depth,
                                                           &c->sel_scratch.p, &c->sel_loc.p)) != DFX_OK)
         return st;
     if (x.side_ao)
@@ -1286,7 +1325,7 @@ dfx_status record_front(const FrameCtx& x, cudaStream_t s, dfx_plane* color_out)
     }
     // DepthRangeCalculator inside the chain (HnComputeDepthBoundsTask, before the post-process task): this frame's range into the
     // frame's camera, which the scene-depth compose below reads
-    if (c->view_mode == DFX_VIEW_MODE_SCENE_DEPTH && (st = dfx_pass_depth_range(s, c->pfx->cams_dev, f->depth, &c->pfx->cams_dev[0].fSceneNearZ)) != DFX_OK)
+    if (ft.view_mode == DFX_VIEW_MODE_SCENE_DEPTH && (st = dfx_pass_depth_range(s, c->pfx->cams_dev, f->depth, &c->pfx->cams_dev[0].fSceneNearZ)) != DFX_OK)
         return st;
     dfx_plane        color = *f->color, ssr_out{}, ao_out{};
     const dfx_plane *pssr = nullptr, *pao = nullptr;
@@ -1304,17 +1343,17 @@ dfx_status record_front(const FrameCtx& x, cudaStream_t s, dfx_plane* color_out)
         }
         // V: HnPostProcess.psh with the view mode's VIEW_MODE. TAA off: drawn into the final target like F. TAA on: TONE_MAPPING_MODE 0,
         // no grid, no sRGB (HnPostProcessTask.cpp:158-231), the selection with its reverse-tone-mapped colours in the same launch
-        if (compose_view_mode(c->view_mode))
+        if (compose_view_mode(ft.view_mode))
         {
             const dfx_selection_attribs* sel = x.sel ? &x.sel_shader : nullptr;
             if (x.final_compose)
-                return dfx_pass_compose_view(s, c->pfx->cams_dev, c->view_mode, c->loading_factor, &color, pssr, pao, cfg.ssr_scale, cfg.ssao_scale, &cfg.tonemap,
-                                             cfg.ave_log_lum, cfg.to_srgb, sel, f->depth, &c->sel_depth, &c->sel_loc.p, &c->mesh_id, c->grid_flags, &c->grid,
+                return dfx_pass_compose_view(s, c->pfx->cams_dev, ft.view_mode, ft.loading_factor, &color, pssr, pao, cfg.ssr_scale, cfg.ssao_scale, &cfg.tonemap,
+                                             cfg.ave_log_lum, cfg.to_srgb, sel, f->depth, &ft.sel_depth, &c->sel_loc.p, &ft.mesh_id, ft.grid_flags, &ft.grid,
                                              f->ldr_out, dfx_rows{0, c->h});
             dfx_tonemap_attribs none = cfg.tonemap;
             none.iToneMappingMode    = DFX_TONE_MAPPING_MODE_NONE;
-            if ((st = dfx_pass_compose_view(s, c->pfx->cams_dev, c->view_mode, c->loading_factor, &color, pssr, pao, cfg.ssr_scale, cfg.ssao_scale, &none,
-                                            cfg.ave_log_lum, 0, sel, f->depth, &c->sel_depth, &c->sel_loc.p, &c->mesh_id, 0, &c->grid, &c->composed.p,
+            if ((st = dfx_pass_compose_view(s, c->pfx->cams_dev, ft.view_mode, ft.loading_factor, &color, pssr, pao, cfg.ssr_scale, cfg.ssao_scale, &none,
+                                            cfg.ave_log_lum, 0, sel, f->depth, &ft.sel_depth, &c->sel_loc.p, &ft.mesh_id, 0, &ft.grid, &c->composed.p,
                                             dfx_rows{0, c->h})) != DFX_OK)
                 return st;
             color = c->composed.p;
@@ -1323,7 +1362,7 @@ dfx_status record_front(const FrameCtx& x, cudaStream_t s, dfx_plane* color_out)
         else if (x.final_compose)
             return dfx_pass_compose_final(s, c->pfx->cams_dev, &color, pssr, pao, x.mv ? 0.0f : cfg.ssr_scale, x.mv ? 0.0f : cfg.ssao_scale, &cfg.tonemap,
                                           cfg.ave_log_lum, cfg.to_srgb,
-                                          x.sel ? &x.sel_shader : nullptr, f->depth, &c->sel_depth, &c->sel_loc.p, c->grid_flags, &c->grid, f->ldr_out,
+                                          x.sel ? &x.sel_shader : nullptr, f->depth, &ft.sel_depth, &c->sel_loc.p, ft.grid_flags, &ft.grid, f->ldr_out,
                                           dfx_rows{0, c->h});
         else if (!x.fuse_compose)
         {
@@ -1331,7 +1370,7 @@ dfx_status record_front(const FrameCtx& x, cudaStream_t s, dfx_plane* color_out)
             color = c->composed.p;
         }
         // O on the composed HDR colour, before TAA (HnPostProcess.psh:211-244 with TONE_MAPPING_MODE 0)
-        if (x.sel && !compose_view_mode(c->view_mode) && (st = dfx_pass_selection_outline(s, &x.sel_shader, f->depth, &c->sel_depth, &c->sel_loc.p, &color, dfx_rows{0, c->h})) != DFX_OK) return st;
+        if (x.sel && !compose_view_mode(ft.view_mode) && (st = dfx_pass_selection_outline(s, &x.sel_shader, f->depth, &ft.sel_depth, &c->sel_loc.p, &color, dfx_rows{0, c->h})) != DFX_OK) return st;
     }
     if (x.st & DFX_CHAIN_STAGE_TAA)
     {
@@ -1355,7 +1394,7 @@ dfx_status record_front(const FrameCtx& x, cudaStream_t s, dfx_plane* color_out)
 // Bloom + ToneMap(+sRGB) on `s`
 dfx_status record_post(const FrameCtx& x, cudaStream_t s, dfx_plane color)
 {
-    dfx_chain*              c   = x.c;
+    const dfx_chain*        c   = x.c;
     const dfx_chain_config& cfg = c->cfg;
     dfx_status              st;
     if (x.final_compose) return DFX_OK;
@@ -1368,14 +1407,100 @@ dfx_status record_post(const FrameCtx& x, cudaStream_t s, dfx_plane color)
     }
     // G2 (HnCopyFrame.psh with ENABLE_GRID) reads the frame's depth and current camera (HnPostProcessTask.cpp:459-475)
     if ((x.st & DFX_CHAIN_STAGE_TONEMAP) && x.grid)
-        return dfx_pass_copy_frame_grid(s, c->pfx->cams_dev, &cfg.tonemap, cfg.ave_log_lum, cfg.to_srgb, c->grid_flags, &c->grid, &color, x.f->depth, x.f->ldr_out,
-                                        dfx_rows{0, c->h});
+        return dfx_pass_copy_frame_grid(s, c->pfx->cams_dev, &cfg.tonemap, cfg.ave_log_lum, cfg.to_srgb, c->ft.grid_flags, &c->ft.grid, &color, x.f->depth,
+                                        x.f->ldr_out, dfx_rows{0, c->h});
     if (x.st & DFX_CHAIN_STAGE_TONEMAP) return dfx_pass_tonemap(s, &cfg.tonemap, cfg.ave_log_lum, cfg.to_srgb, &color, x.f->ldr_out, dfx_rows{0, c->h});
     return DFX_OK;
 }
 
-// what TAA's output plane will be for this frame (needed by the replay path, which never calls record_front)
+// the effect's alpha no longer changes: pinned, or its fade-in is over
 bool alpha_constant(AlphaTimer& a) { return a.pinned >= 0.0f || a.value() >= 1.0f; }
+
+// Can this frame be replayed from a graph: consecutive frame indices, no history reset, constant attributes
+bool steady(const FrameCtx& x)
+{
+    const dfx_chain*        c   = x.c;
+    const dfx_chain_config& cfg = c->cfg;
+    const TaaBuffer&        b   = c->taa->buffers[0];
+    return cfg.use_graph && c->graphs_ok && !profiling_enabled() && c->last_frame != ~0u && x.f->frame_index == c->last_frame + 1u &&
+           (!(x.st & DFX_CHAIN_STAGE_SSAO) || (c->ssao->last_frame != ~0u && c->ssao->curr_frame == c->ssao->last_frame + 1u && !cfg.ssao.ResetAccumulation &&
+                                               alpha_constant(c->ssao->alpha))) &&
+           (!(x.st & DFX_CHAIN_STAGE_SSR) || alpha_constant(c->ssr->alpha)) && (!(x.st & DFX_CHAIN_STAGE_BLOOM) || alpha_constant(c->bloom->alpha)) &&
+           (!x.with_dof || alpha_constant(c->dof->alpha)) &&
+           (!(x.st & DFX_CHAIN_STAGE_TAA) || (b.last_frame != ~0u && b.curr_frame == b.last_frame + 1u && !cfg.taa.ResetAccumulation && !x.taa_reset));
+}
+
+// The graph cache's key: everything a recorded launch reads from the host, for what this frame runs
+std::string graph_key(const FrameCtx& x)
+{
+    const dfx_chain*       c  = x.c;
+    const ChainFeatures&   ft = c->ft;
+    const dfx_chain_frame* f  = x.f;
+    const uint32_t         par = f->frame_index & 1u;
+    std::string            key;
+    key.reserve(1024);
+    append(key, par, c->cfg);
+    for (const dfx_plane* p : {f->depth, f->prev_depth, f->motion, f->normal, f->color, f->material, f->ldr_out}) append_plane(key, p);
+    const float alphas[4] = {c->ssao->alpha.value(), c->ssr->alpha.value(), c->bloom->alpha.value(), c->dof->alpha.value()};
+    append(key, alphas);
+    if (x.grid) append(key, ft.grid_flags, ft.grid);
+    if (x.env) append(key, ft.env_type, ft.env_map, ft.env_options, ft.env);
+    if (x.box) append(key, 'B', ft.box);
+    if (x.debug) append(key, ft.view_mode, ft.mesh_id);
+    if (x.debug && ft.view_mode == DFX_VIEW_MODE_SCENE_DEPTH) append(key, ft.loading_factor);
+    if (x.sel)
+    {
+        dfx_selection_attribs k = x.sel_shader;
+        k.selection_id          = 0; // the id only decides when TAA resets, which is never a replayed frame
+        append(key, k, ft.sel_depth);
+    }
+    return key;
+}
+
+// The frame's graphs, captured on the chain's own stream (the caller's may be the legacy default stream, which cannot capture): the
+// front half, with the back half unless that runs on the third stream, then the back half. False: a capture failed.
+bool record_graphs(const FrameCtx& x, GraphPair& g)
+{
+    const cudaStream_t s = x.c->cap_stream;
+    dfx_plane          color{};
+    const auto         capture = [&](cudaGraphExec_t* exec, bool front, bool post) {
+        cudaGraph_t graph = nullptr;
+        cudaError_t e     = cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
+        dfx_status  rs    = e == cudaSuccess ? DFX_OK : check_cuda(e, "cudaStreamBeginCapture");
+        if (rs == DFX_OK && front) rs = record_front(x, s, &color);
+        if (rs == DFX_OK && post) rs = record_post(x, s, color);
+        if (e == cudaSuccess) e = cudaStreamEndCapture(s, &graph);
+        if (rs == DFX_OK && e == cudaSuccess) e = cudaGraphInstantiate(exec, graph, 0);
+        if (graph) cudaGraphDestroy(graph);
+        return rs == DFX_OK && e == cudaSuccess;
+    };
+    return capture(&g.front, true, !x.side_post) && (!x.side_post || capture(&g.post, false, true));
+}
+
+// The frame's graphs, recorded the first time its key is seen; null: the frame is issued eagerly
+GraphPair* graphs_for(dfx_chain* c, const FrameCtx& x)
+{
+    if (!steady(x)) return nullptr;
+    const std::string key = graph_key(x);
+    GraphPair&        g   = c->graphs[key];
+    if (g.front) return &g;
+    const uint64_t counted0 = dfx_launch_count();
+    bool           ok       = record_graphs(x, g);
+    if (ok)
+        c->stats.graphs_built += 1, g.kernels = int(dfx_launch_count() - counted0);
+    else
+    {
+        // a capture that failed leaves nothing on the GPU: run this frame (and every later one) eagerly
+        (void)cudaGetLastError();
+        if (g.front) cudaGraphExecDestroy(g.front);
+        if (g.post) cudaGraphExecDestroy(g.post);
+        c->graphs.erase(key);
+        c->graphs_ok = false, c->stats.graph_failures += 1;
+    }
+    count_launch(-int(dfx_launch_count() - counted0)); // recorded, not launched
+    if (c->graphs.size() > 64) c->drop_graphs(), ok = false; // runaway key churn (a caller that never reuses its planes): stay eager
+    return ok ? &g : nullptr;
+}
 } // namespace
 
 extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_chain_frame* f)
@@ -1384,41 +1509,10 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
     DFX_REQUIRE(f->curr_camera && f->prev_camera, "camera attribs must not be null");
     DFX_REQUIRE(f->depth && f->prev_depth && f->motion && f->normal && f->color && f->material, "all six G-buffer planes must be given");
     const dfx_chain_config& cfg = c->cfg;
-    // With TAA off there is no TAA, hence no Bloom and no DepthOfField (HnPostProcessTask.cpp:652-654). A debug view mode runs no SSR,
-    // SSAO, Bloom or DepthOfField (:625-654), and PostFX only where TAA runs (:788)
-    const bool debug = debug_view(c->view_mode);
-    // The motion-vector view switches TAA off (:652) and with it PostFX (:788): F draws the frame, the vector field goes over it
-    const bool mv = c->view_mode == DFX_VIEW_MODE_MOTION_VECTORS;
-    uint32_t   st = cfg.disable_taa || mv ? cfg.stages & ~(DFX_CHAIN_STAGE_TAA | DFX_CHAIN_STAGE_BLOOM) : cfg.stages;
-    if (debug) st &= ~(DFX_CHAIN_STAGE_SSR | DFX_CHAIN_STAGE_SSAO | DFX_CHAIN_STAGE_BLOOM | (cfg.disable_taa || mv ? DFX_CHAIN_STAGE_POSTFX : 0u));
+    FrameCtx                x   = plan_frame(*c, *f);
+    const uint32_t          st  = x.st;
     DFX_REQUIRE(!(st & (DFX_CHAIN_STAGE_TONEMAP)) || f->ldr_out, "the tone-mapped output plane must be given");
     cudaStream_t main = as_stream(stream);
-    FrameCtx     x{c, f, st, false, false, false, false, false, false, false, false, false, {}, false, debug};
-    // With the grid on, its step reads the caller's depth plane and the camera of this frame: Bloom + the grid step stay on the
-    // caller's stream, in order with what the caller does to its planes next, and the Bloom composite runs unfused before it.
-    x.grid          = c->grid_flags != 0;
-    x.env           = c->env_on && c->view_mode != DFX_VIEW_MODE_SCENE_DEPTH; // HnRenderEnvMapTask::IsActive (HnRenderEnvMapTask.cpp:85-94)
-    x.box           = c->box_on; // HnRenderBoundBoxTask has no IsActive: every view mode
-    x.mv            = mv;
-    x.final_compose = cfg.disable_taa != 0 || mv;
-    x.with_dof      = cfg.enable_dof != 0 && !x.final_compose && !debug;
-    x.side_ao      = cfg.overlap && (st & DFX_CHAIN_STAGE_SSAO) && (st & DFX_CHAIN_STAGE_SSR);
-    x.side_post    = cfg.overlap && (st & DFX_CHAIN_STAGE_BLOOM) && (st & DFX_CHAIN_STAGE_TAA) && !x.with_dof && !x.grid;
-    // With selection on, O runs between the compose and TAA: the compose runs unfused
-    x.sel          = c->sel_on;
-    x.taa_reset    = c->sel_taa_reset;
-    x.fuse_compose = cfg.fuse && (st & DFX_CHAIN_STAGE_COMPOSE) && (st & DFX_CHAIN_STAGE_TAA) && !x.sel && !compose_view_mode(c->view_mode);
-    if (x.sel)
-    {
-        // HnPostProcessTask.cpp:840-850: with TAA on and a tone map after it, the outline colours are reverse-tone-mapped
-        x.sel_shader = c->sel;
-        if (!x.final_compose && cfg.tonemap.iToneMappingMode != DFX_TONE_MAPPING_MODE_NONE)
-        {
-            dfx_reverse_exp_tone_map(c->sel.SelectionColor, cfg.tonemap.fMiddleGray, cfg.ave_log_lum, x.sel_shader.SelectionColor);
-            dfx_reverse_exp_tone_map(c->sel.OccludedSelectionColor, cfg.tonemap.fMiddleGray, cfg.ave_log_lum, x.sel_shader.OccludedSelectionColor);
-        }
-    }
-    x.fuse_tonemap = cfg.fuse && (st & DFX_CHAIN_STAGE_BLOOM) && (st & DFX_CHAIN_STAGE_TONEMAP) && (c->w % 2 == 0) && (c->h % 2 == 0) && !x.grid;
     // launch shapes that depend on whether the two halves of the frame share the GPU (dfx_pyramid.cuh: build_pyramid) read this while
     // the frame is issued or recorded; it is part of the graph key through cfg.overlap
     struct AsyncHint
@@ -1439,144 +1533,49 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
     if ((st & DFX_CHAIN_STAGE_COMPOSE) && !x.fuse_compose && !x.final_compose && !c->composed.p.ptr && (s = c->composed.alloc(c->w, c->h, DFX_FORMAT_RGBA32F)) != DFX_OK) return s;
     for (PlaneOwner* p : {&c->sel_loc, &c->sel_scratch})
         if (x.sel && !p->p.ptr && (s = p->alloc(c->w, c->h, DFX_FORMAT_RG32F)) != DFX_OK) return s;
-    if (mv && !c->mv_owner.p.ptr)
+    if (x.mv && !c->mv_owner.p.ptr)
     {
         if ((s = c->mv_owner.alloc(c->w, c->h, DFX_FORMAT_R32F)) != DFX_OK) return s;
         DFX_CUDA(cudaMemsetAsync(c->mv_owner.p.ptr, 0, c->mv_owner.p.pitch_bytes * size_t(c->h), main));
     }
-    // the front pass needs every pass it replaces in this frame, at full resolution; dfx_tune "front_fused" = 0 keeps the separate passes
-    const uint32_t front_stages = DFX_CHAIN_STAGE_POSTFX | DFX_CHAIN_STAGE_SSR | DFX_CHAIN_STAGE_SSAO;
-    x.front = cfg.fuse && (st & front_stages) == front_stages && !(cfg.ssr_flags & DFX_SSR_FEATURE_FLAG_HALF_RESOLUTION) &&
-              !(cfg.ssao_flags & DFX_SSAO_FEATURE_FLAG_HALF_RESOLUTION) && dfx_tune_get("front_fused", 1) &&
-              front_prepare_fusable(f->depth, c->ssr->levels, c->ssao->levels);
+    x.front = x.front && front_prepare_fusable(f->depth, c->ssr->levels, c->ssao->levels);
 
-    // ---- can this frame be replayed from a graph?
-    const uint32_t par    = f->frame_index & 1u;
-    bool           steady = cfg.use_graph && c->graphs_ok && !profiling_enabled() && c->last_frame != ~0u && f->frame_index == c->last_frame + 1u;
-    if (steady && (st & DFX_CHAIN_STAGE_SSAO))
-        steady = c->ssao->last_frame != ~0u && c->ssao->curr_frame == c->ssao->last_frame + 1u && !cfg.ssao.ResetAccumulation && alpha_constant(c->ssao->alpha);
-    if (steady && (st & DFX_CHAIN_STAGE_SSR)) steady = alpha_constant(c->ssr->alpha);
-    if (steady && (st & DFX_CHAIN_STAGE_BLOOM)) steady = alpha_constant(c->bloom->alpha);
-    if (steady && x.with_dof) steady = alpha_constant(c->dof->alpha);
-    if (steady && (st & DFX_CHAIN_STAGE_TAA))
-    {
-        const TaaBuffer& b = c->taa->buffers[0];
-        steady             = b.last_frame != ~0u && b.curr_frame == b.last_frame + 1u && !cfg.taa.ResetAccumulation && !x.taa_reset;
-    }
-
-    // ---- TAA of this frame overwrites the accumulator that Bloom of frame f-2 read on the chain's third stream
-    if (c->post_pending[par])
-    {
-        DFX_CUDA(cudaStreamWaitEvent(main, c->post_done[par], 0));
-        c->post_pending[par] = false;
-    }
-    // ---- the grid was switched on, TAA off or a debug view mode on, after a frame that left its Bloom + ToneMap running on the chain's
-    // third stream: this frame's grid step, F, V or tone map writes the LDR plane on `main`
-    for (int i = 0; i < 2 && (x.grid || x.final_compose || debug); ++i)
-        if (c->post_pending[i])
+    // ---- TAA of this frame overwrites the accumulator that Bloom of frame f-2 read on the chain's third stream; with the grid, TAA off or
+    // a debug view, this frame's grid step, F, V or tone map writes the LDR plane on `main` that a Bloom + ToneMap there may still write
+    const uint32_t par = f->frame_index & 1u;
+    for (uint32_t i = 0; i < 2; ++i)
+        if (c->post_pending[i] && (i == par || x.grid || x.final_compose || x.debug))
         {
             DFX_CUDA(cudaStreamWaitEvent(main, c->post_done[i], 0));
             c->post_pending[i] = false;
         }
     // ---- cameras + frame index -> device memory (kernel parameters, no copy engine; outside the recorded graphs: they change every frame)
-    if (((st & DFX_CHAIN_STAGE_POSTFX) || x.grid || x.env || x.box || compose_view_mode(c->view_mode)) && (s = launch_upload_cameras(main, f->curr_camera, f->prev_camera, f->frame_index, c->pfx->cams_dev, c->pfx->frame_dev)) != DFX_OK) return s;
+    if (x.upload_cameras && (s = launch_upload_cameras(main, f->curr_camera, f->prev_camera, f->frame_index, c->pfx->cams_dev, c->pfx->frame_dev)) != DFX_OK) return s;
 
-    dfx_plane color{};
-    bool      replayed = false;
-    if (steady)
+    // ---- the front half on `main`, then the back half on the chain's third stream or after it: replayed from graphs or issued
+    GraphPair* g = graphs_for(c, x);
+    dfx_plane  color{};
+    if (g)
+        DFX_CUDA(cudaGraphLaunch(g->front, main));
+    else if ((s = record_front(x, main, &color)) != DFX_OK)
+        return s;
+    if (x.side_post)
     {
-        std::string key;
-        key.reserve(1024);
-        append_bytes(key, &par, sizeof(par));
-        append_bytes(key, &cfg, sizeof(cfg));
-        for (const dfx_plane* p : {f->depth, f->prev_depth, f->motion, f->normal, f->color, f->material, f->ldr_out}) append_plane(key, p);
-        const float alphas[4] = {c->ssao->alpha.value(), c->ssr->alpha.value(), c->bloom->alpha.value(), c->dof->alpha.value()};
-        append_bytes(key, alphas, sizeof(alphas));
-        if (x.grid) append_bytes(key, &c->grid_flags, sizeof(c->grid_flags)), append_bytes(key, &c->grid, sizeof(c->grid));
-        if (x.env)
-        {
-            append_bytes(key, &c->env_type, sizeof(c->env_type)), append_bytes(key, &c->env_map, sizeof(c->env_map));
-            append_bytes(key, &c->env_options, sizeof(c->env_options)), append_bytes(key, &c->env, sizeof(c->env));
-        }
-        if (x.box) key.push_back('B'), append_bytes(key, &c->box, sizeof(c->box));
-        if (debug)
-        {
-            append_bytes(key, &c->view_mode, sizeof(c->view_mode)), append_plane(key, &c->mesh_id);
-            if (c->view_mode == DFX_VIEW_MODE_SCENE_DEPTH) append_bytes(key, &c->loading_factor, sizeof(c->loading_factor));
-        }
-        if (x.sel)
-        {
-            dfx_selection_attribs k = x.sel_shader;
-            k.selection_id          = 0; // the id only decides when TAA resets, which is never a replayed frame
-            append_bytes(key, &k, sizeof(k)), append_plane(key, &c->sel_depth);
-        }
-        GraphPair& g = c->graphs[key];
-        if (!g.front)
-        {
-            // capture on the chain's own stream (the caller's may be the legacy default stream, which cannot capture)
-            cudaGraph_t    graph    = nullptr;
-            const uint64_t counted0 = dfx_launch_count();
-            cudaError_t    e        = cudaStreamBeginCapture(c->cap_stream, cudaStreamCaptureModeThreadLocal);
-            dfx_status  rs    = e == cudaSuccess ? record_front(x, c->cap_stream, &color) : check_cuda(e, "cudaStreamBeginCapture");
-            if (rs == DFX_OK && !x.side_post) rs = record_post(x, c->cap_stream, color);
-            if (e == cudaSuccess) e = cudaStreamEndCapture(c->cap_stream, &graph);
-            if (rs == DFX_OK && e == cudaSuccess) e = cudaGraphInstantiate(&g.front, graph, 0);
-            if (graph) cudaGraphDestroy(graph);
-            if (rs == DFX_OK && e == cudaSuccess && x.side_post)
-            {
-                graph = nullptr;
-                e     = cudaStreamBeginCapture(c->cap_stream, cudaStreamCaptureModeThreadLocal);
-                rs    = e == cudaSuccess ? record_post(x, c->cap_stream, color) : check_cuda(e, "cudaStreamBeginCapture");
-                if (e == cudaSuccess) e = cudaStreamEndCapture(c->cap_stream, &graph);
-                if (rs == DFX_OK && e == cudaSuccess) e = cudaGraphInstantiate(&g.post, graph, 0);
-                if (graph) cudaGraphDestroy(graph);
-            }
-            if (rs != DFX_OK || e != cudaSuccess)
-            {
-                // a capture that failed leaves nothing on the GPU: run this frame (and every later one) eagerly
-                (void)cudaGetLastError();
-                if (g.front) cudaGraphExecDestroy(g.front);
-                if (g.post) cudaGraphExecDestroy(g.post);
-                c->graphs.erase(key);
-                c->graphs_ok = false;
-                c->stats.graph_failures += 1;
-                steady = false;
-            }
-            else
-            {
-                c->stats.graphs_built += 1;
-                g.kernels = int(dfx_launch_count() - counted0);
-            }
-            count_launch(-int(dfx_launch_count() - counted0)); // recorded, not launched
-            if (c->graphs.size() > 64) c->drop_graphs(), steady = false; // runaway key churn (a caller that never reuses its planes): stay eager
-        }
-        if (steady)
-        {
-            GraphPair& gg = c->graphs[key];
-            DFX_CUDA(cudaGraphLaunch(gg.front, main));
-            if (x.side_post)
-            {
-                DFX_CUDA(cudaEventRecord(c->ev_front_done, main));
-                DFX_CUDA(cudaStreamWaitEvent(c->post_stream, c->ev_front_done, 0));
-                DFX_CUDA(cudaGraphLaunch(gg.post, c->post_stream));
-            }
-            // the host-side state the effects' Execute() would have advanced
-            c->pfx->executed = true;
-            if (st & DFX_CHAIN_STAGE_SSAO) c->ssao->last_frame = c->ssao->curr_frame;
-            if (st & DFX_CHAIN_STAGE_TAA) c->taa->buffers[0].last_frame = c->taa->buffers[0].curr_frame;
-            count_launch(gg.kernels);
-            c->stats.frames_replayed += 1;
-            replayed = true;
-        }
+        DFX_CUDA(cudaEventRecord(c->ev_front_done, main));
+        DFX_CUDA(cudaStreamWaitEvent(c->post_stream, c->ev_front_done, 0));
     }
-    if (!replayed)
+    if (g)
     {
-        if ((s = record_front(x, main, &color)) != DFX_OK) return s;
-        if (x.side_post)
-        {
-            DFX_CUDA(cudaEventRecord(c->ev_front_done, main));
-            DFX_CUDA(cudaStreamWaitEvent(c->post_stream, c->ev_front_done, 0));
-        }
+        if (x.side_post) DFX_CUDA(cudaGraphLaunch(g->post, c->post_stream));
+        // the host-side state the effects' Execute() would have advanced
+        c->pfx->executed = true;
+        if (st & DFX_CHAIN_STAGE_SSAO) c->ssao->last_frame = c->ssao->curr_frame;
+        if (st & DFX_CHAIN_STAGE_TAA) c->taa->buffers[0].last_frame = c->taa->buffers[0].curr_frame;
+        count_launch(g->kernels);
+        c->stats.frames_replayed += 1;
+    }
+    else
+    {
         if ((s = record_post(x, x.side_post ? c->post_stream : main, color)) != DFX_OK) return s;
         c->stats.frames_eager += 1;
     }
@@ -1591,10 +1590,10 @@ extern "C" dfx_status dfx_chain_execute(dfx_chain* c, void* stream, const dfx_ch
         }
     }
     // the vector field over the final frame (HnPostProcessTask.cpp:928-943), outside the graph: its scale changes every frame
-    if (mv)
+    if (x.mv)
     {
         dfx_vector_field_attribs va;
-        dfx_vector_field_attribs_hydrogent(uint32_t(c->w), uint32_t(c->h), c->mv_elapsed, &va);
+        dfx_vector_field_attribs_hydrogent(uint32_t(c->w), uint32_t(c->h), c->ft.mv_elapsed, &va);
         if ((s = dfx_pass_vector_field(main, &va, cfg.to_srgb ? DFX_VECTOR_FIELD_OPTION_CONVERT_OUTPUT_TO_SRGB : 0u, f->motion, f->ldr_out, &c->mv_owner.p,
                                        dfx_rows{0, c->h})) != DFX_OK)
             return s;
